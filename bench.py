@@ -1,6 +1,7 @@
-"""bench.py — driver contract (see task statement): one JSON line per run.
+"""bench.py — measures the flagship workload and prints one JSON line per run.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload e2e|align] [--impl ours|reference]
+                    [--dump-outputs DIR]
 
 Workloads
   e2e   : (default) BASELINE.json metric — audio-seconds/second of whisper_timestamped.transcribe() for
@@ -8,7 +9,11 @@ Workloads
           timestamps + confidences on; N GPUs shard the chunks (strong scaling) and gather the JSON.
   align : SURVEY.md §8(d) alignment micro-benchmark — a batch of synthetic alignment problems
           (N=10 heads, qk ~ 3*N(0,1) + monotone ridge) through wts_attn_prep_batch +
-          wts_dtw_batch; reports the DTW kernel's algorithmic GB/s against the measured HBM peak.
+          wts_dtw_batch; reports the DTW kernel's algorithmic GB/s against the HBM peak.
+
+--dump-outputs DIR writes what the timed path returned in its last timed step as DIR/<name>.npy (float64, 64 MB at
+most: a larger output is written as a fixed seeded sample), so that two builds can be compared output for output: the
+inputs are seeded and identical from run to run.
 """
 import argparse
 import json
@@ -34,7 +39,8 @@ def measured_peaks():
         return {"hbm_gbs": float(d["hbm_gbs"]), "bf16_tflops": float(d["bf16_tflops"]),
                 "bf16_tflops_sustained": float(d.get("bf16_tflops_sustained", d["bf16_tflops"])),
                 "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "data sheet (H100 SXM)"}
 
 
 class ClockSampler:
@@ -121,15 +127,6 @@ def bytes_prep(N, T, F):
     return 4 * N * T * F + 4 * T * F
 
 
-def dtw_traffic(kernel):
-    """dram read + write bytes of one launch from the committed ncu capture (profiles/roofline_traffic.json), or None."""
-    try:
-        t = json.load(open(os.path.join(ROOT, "profiles", "roofline_traffic.json")))[kernel]
-        return int(t["dram_bytes_read"]) + int(t["dram_bytes_write"])
-    except Exception:                                          # noqa: BLE001
-        return None
-
-
 def dtw_kernel_name(nseg, T):
     """Which DTW kernel wts_dtw_batch_sized picks for a batch of nseg single-strip matrices (csrc/dtw.cu)."""
     lane_min = int(os.environ.get("WTS_DTW_LANE_MIN", "8192"))
@@ -189,6 +186,9 @@ def run_align(args, rank, world):
     wall = time.perf_counter() - t0
     total_ms = e0.elapsed_time(e1)
     clocks = sampler.stop() if rank == 0 else None
+    # what the last timed step computed, copied out before the host-buffer loop below reuses the cost buffer
+    dumped = (align_dump_arrays(out["jumps"], cost, nseg, T)
+              if rank == 0 and args.dump_outputs and args.workload == "align" else None)
     # host-buffer e2e: qk slices are device-resident products of the decoder in the real pipeline, so the
     # host-facing e2e of this micro-workload = descriptors H2D + jumps D2H each step
     e2e_t = []
@@ -212,6 +212,7 @@ def run_align(args, rank, world):
         "e2e_segments_per_s": nseg / float(np.median(e2e_t)),
         "h2d": int(plan.segs.nbytes), "d2h": int(plan.jumps_elems * 4),
         "peaks": peaks, "alg_bytes": alg, "jumps_checksum": int(out["jumps"].sum().item()),
+        "outputs": dumped,
     }
     return res
 
@@ -287,7 +288,7 @@ def make_audio(seconds, seed=1234):
 def gemm_roofline(engine, peaks, reps=20):
     """Dominant kernel = gemm_tc_kernel.  Times the encoder MLP up-projection shape (the largest FLOP share)
     alone with CUDA events; algorithmic flops = 2*M*N*K (one float32-accurate product; the kernel issues three
-    bf16 UMMAs per product)."""
+    bf16 wgmmas per product)."""
     import torch
     from whisper_timestamped.model import SB16
     d = engine.dims
@@ -309,17 +310,9 @@ def gemm_roofline(engine, peaks, reps=20):
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / reps
     tf = 2.0 * M * N * K / (ms * 1e-3) / 1e12
-    traffic = None
-    try:        # DRAM bytes of one launch of this shape from the committed ncu --set full capture
-        t = json.load(open(os.path.join(ROOT, "profiles", "roofline_traffic.json")))["gemm_tc_persist_kernel"]
-        if t["shape"] == [M, N, K]:
-            traffic = t["dram_bytes_read"] + t["dram_bytes_write"]
-    except (OSError, KeyError, ValueError):
-        pass
     return {"bound": "tensor", "achieved": tf, "peak": peaks["bf16_tflops"], "unit": "TFLOP/s",
-            "frac": tf / peaks["bf16_tflops"], "traffic": traffic, "traffic_unit": "bytes per launch (dram read + write, ncu)",
-            "peak_source": peaks["source"],
-            "kernel": "gemm_tc_persist_kernel (bf16x3: 3 UMMAs per float32-accurate product; tensor-pipe work = 3x achieved)",
+            "frac": tf / peaks["bf16_tflops"], "peak_source": peaks["source"],
+            "kernel": "gemm_tc_kernel (bf16x3: 3 wgmmas per float32-accurate product; tensor-pipe work = 3x achieved)",
             "shape": [M, N, K], "ms": ms}
 
 
@@ -365,6 +358,7 @@ def run_e2e(args, rank, world, local):
     for _ in range(args.steps):
         res = one(dev_audio)
     e1.record()
+    timed_res = res
     barrier()
     wall = time.perf_counter() - t0
     ms = e0.elapsed_time(e1)
@@ -397,7 +391,7 @@ def run_e2e(args, rank, world, local):
            "clocks": clocks, "launches": launches, "segments": len(res["segments"]), "tokens": ntok, "words": nw,
            "h2d": int(mine.nbytes), "d2h": int(len(json.dumps(res["segments"]))) if rank == 0 else 0, "wall_s": wall,
            "decode_steps": getattr(eng, "decode_steps_run", 0), "small_batch_steps": eng.small_batch_steps,
-           "result": res if rank == 0 else None}
+           "result": res if rank == 0 else None, "timed_result": timed_res if rank == 0 else None}
     if rank == 0 and not args.no_roofline:
         peaks = measured_peaks()
         out["roofline"] = gemm_roofline(eng, peaks)
@@ -554,6 +548,66 @@ def parity_vs_reference(ours, ref_results, timed, chunk_seconds):
             "max_word_dt": round(max_dt, 6), "max_confidence_diff": round(max_dc, 6)}
 
 
+DUMP_LIMIT = 64 << 20          # bytes of .npy data --dump-outputs may write
+
+
+def _write_dump(out_dir, arrays):
+    total = sum(a.nbytes for a in arrays.values())
+    assert total <= DUMP_LIMIT, f"--dump-outputs: {total} bytes exceed {DUMP_LIMIT}"   # the callers sample to fit
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
+def _seeded_subset(n, keep):
+    """Sorted indices of a fixed seeded sample of `keep` out of `n` items (all of them when keep >= n)."""
+    if keep >= n:
+        return np.arange(n)
+    return np.sort(np.random.default_rng(0).choice(n, size=keep, replace=False))
+
+
+def _e2e_arrays(segs, index):
+    f64 = lambda x: np.asarray(x, dtype=np.float64)
+    segs = [segs[i] for i in index]
+    words = [w for s in segs for w in s.get("words", [])]
+    return {
+        "segment_index": f64(index),
+        "tokens": f64([t for s in segs for t in s["tokens"]]),
+        "segment_tokens": f64([len(s["tokens"]) for s in segs]),
+        "segment_seek": f64([s["seek"] for s in segs]),
+        "segment_times": f64([[s["start"], s["end"]] for s in segs]).reshape(-1, 2),
+        "segment_scores": f64([[s["avg_logprob"], s["compression_ratio"], s["no_speech_prob"], s.get("confidence", np.nan),
+                                s["temperature"]] for s in segs]).reshape(-1, 5),
+        "segment_words": f64([len(s.get("words", [])) for s in segs]),
+        "word_times": f64([[w["start"], w["end"]] for w in words]).reshape(-1, 2),
+        "word_confidence": f64([w["confidence"] for w in words]),
+    }
+
+
+def dump_e2e_outputs(out_dir, res):
+    """What transcribe() returned: the tokens, per-segment numbers and per-word times / confidences, in order.  When
+    that exceeds DUMP_LIMIT, a fixed seeded sample of whole segments (their indices in `segment_index`)."""
+    segs = res["segments"]
+    keep = len(segs)
+    arrays = _e2e_arrays(segs, _seeded_subset(len(segs), keep))
+    while sum(a.nbytes for a in arrays.values()) > DUMP_LIMIT:
+        keep = int(keep * 0.9)
+        arrays = _e2e_arrays(segs, _seeded_subset(len(segs), keep))
+    _write_dump(out_dir, arrays)
+
+
+def align_dump_arrays(jumps, cost, nseg, T, n_sample=1 << 20):
+    """The DTW jumps of every segment (a fixed seeded sample of segments when they exceed half of DUMP_LIMIT) and a
+    fixed seeded sample of the cost matrices (the whole cost buffer exceeds the limit), as host float64 arrays."""
+    import torch
+    idx = _seeded_subset(cost.numel(), min(n_sample, cost.numel()))
+    sample = cost[torch.from_numpy(idx).to(cost.device)].cpu().numpy()
+    rows = jumps.cpu().numpy().astype(np.float64).reshape(nseg, T + 1)
+    seg = _seeded_subset(nseg, (DUMP_LIMIT // 2) // (8 * (T + 1)))
+    return {"jumps": rows[seg], "jumps_segment_index": seg.astype(np.float64),
+            "cost_sample_index": idx.astype(np.float64), "cost_sample": sample.astype(np.float64)}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -564,7 +618,9 @@ def main():
     ap.add_argument("--model", default="large-v3")
     ap.add_argument("--audio-seconds", type=float, default=3600.0)
     ap.add_argument("--chunk-seconds", type=float, default=30.0)
-    ap.add_argument("--max-batch", type=int, default=128)
+    # 64 windows decoded together: the decoder state of 128 large-v3 windows (cross K/V, alignment-head K, self KV)
+    # plus the encoder scratch of one batch does not fit the 80 GB of an H100
+    ap.add_argument("--max-batch", type=int, default=64)
     ap.add_argument("--cpu-seconds", type=float, default=60.0)
     ap.add_argument("--align-batch", type=int, default=16384)
     ap.add_argument("--align-T", type=int, default=24)
@@ -572,7 +628,11 @@ def main():
     ap.add_argument("--recipe", default="default", choices=sorted(RECIPES))
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-roofline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float64, 64 MB at most)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs writes what this project's timed path computed; it has no meaning with --impl reference")
     args.warmup = max(args.warmup, 3)
     SYNTH_KW.clear()
     SYNTH_KW.update(RECIPES[args.recipe])
@@ -580,7 +640,7 @@ def main():
 
     workload_name = (f"{args.model}, {args.audio_seconds:.0f} s synthetic 16 kHz audio in independent "
                      f"{args.chunk_seconds:.0f}-s chunks, greedy, word timestamps + confidences")
-    metric_name = "audio-sec/s (RTF) large-v3 1h synthetic @1/2/4/8 B200; DTW GB/s vs HBM peak"
+    metric_name = "audio-sec/s (RTF) large-v3 1h synthetic @1/2/4/8 H100; DTW GB/s vs HBM peak"
     # identical in both arms (the driver compares them): what is computed, not how
     e2e_config = {"workload": workload_name, "model": args.model, "audio_seconds": args.audio_seconds,
                   "chunk_seconds": args.chunk_seconds, "decoding": "greedy, temperature 0, chunks independent",
@@ -647,12 +707,13 @@ def main():
                     al = run_align(args, rank, world)
                     line["dtw_roofline"] = {
                         "bound": "hbm", "achieved": al["dtw_gbs"], "peak": al["peaks"]["hbm_gbs"], "unit": "GB/s",
-                        "frac": al["dtw_gbs"] / al["peaks"]["hbm_gbs"], "traffic": dtw_traffic(dtw_kernel_name(args.align_batch, args.align_T))
-                        if (args.align_batch, args.align_T, args.align_F) == (16384, 24, 300) else None,
+                        "frac": al["dtw_gbs"] / al["peaks"]["hbm_gbs"],
                         "kernel": dtw_kernel_name(args.align_batch, args.align_T), "ms": al["ms_dtw"], "prep_gbs": al["prep_gbs"], "prep_ms": al["ms_prep"],
                         "workload": f"{args.align_batch} segments, T={args.align_T}, F={args.align_F}, N=10 heads"}
                 except Exception as err:                                   # noqa: BLE001
                     line["dtw_roofline"] = {"error": f"{type(err).__name__}: {err}"[:200]}
+            if args.dump_outputs:
+                dump_e2e_outputs(args.dump_outputs, res["timed_result"])
             if not args.no_cpu_baseline:
                 cb = cpu_baseline_e2e(args)
                 # the reference's own output on those chunks (computed on this box a moment ago) vs ours
@@ -662,6 +723,8 @@ def main():
             print(json.dumps(line))
     else:
         res = run_align(args, rank, world)
+        if rank == 0 and args.dump_outputs:
+            _write_dump(args.dump_outputs, res["outputs"])
         vals = [res["segments_per_s"]]
         ms = [res["ms_total"]]
         if world > 1:
@@ -682,8 +745,6 @@ def main():
                            "l2": "inputs (qk %.1f GB) larger than L2" % (args.align_batch * 10 * args.align_T * 1500 * 4 / 1e9)},
                 "roofline": {"bound": "hbm", "achieved": res["dtw_gbs"], "peak": peaks["hbm_gbs"], "unit": "GB/s",
                              "frac": res["dtw_gbs"] / peaks["hbm_gbs"],
-                             "traffic": dtw_traffic(dtw_kernel_name(args.align_batch, args.align_T))
-                             if (args.align_batch, args.align_T, args.align_F) == (16384, 24, 300) else None,
                              "peak_source": peaks["source"],
                              "kernel": dtw_kernel_name(args.align_batch, args.align_T), "ms": res["ms_dtw"]},
                 "prep": {"gbs": res["prep_gbs"], "ms": res["ms_prep"]},

@@ -1,5 +1,5 @@
 /*
- * libwts — C-ABI of the B200-native word-alignment hot path of whisper-timestamped.
+ * libwts — C-ABI of the H100-native word-alignment hot path of whisper-timestamped.
  *
  * Conventions (all entry points):
  *   - every pointer named d_* is a DEVICE pointer owned by the caller (PyTorch allocations are
@@ -7,7 +7,7 @@
  *     the persistent objects created by *_create and freed by *_destroy;
  *   - `stream` is a cudaStream_t passed as void*; work is enqueued asynchronously on it;
  *   - return value: 0 = OK, <0 = error (message via wts_last_error(), thread-local);
- *   - no C++ exception crosses the ABI; there is no CPU fallback: if no sm_100 device code can
+ *   - no C++ exception crosses the ABI; there is no CPU fallback: if no sm_90a device code can
  *     run, the call fails with an error.
  *
  * Each entry cites the reference interface it replaces
@@ -138,7 +138,7 @@ typedef struct WtsGemm {
     void*  out_sb16;  int64_t ldo, o_plane, o_bo, o_bi; /* SB16 output (may be NULL) */
     int32_t head_dim; int64_t head_stride;   /* if head_dim > 0 output column n goes to
                                                 (n / head_dim) * head_stride + m * ld + (n % head_dim) */
-    int32_t backend;          /* 0 = tcgen05 tensor cores, 1 = SIMT float32 validator */
+    int32_t backend;          /* 0 = wgmma tensor cores, 1 = SIMT float32 validator */
     int32_t a_is_f32, b_is_f32;   /* SIMT backend only: operand is plain float32 (log-mel DFT / filterbank GEMMs) */
     const int32_t* row_mask;  /* optional [M] (M <= 128, unbatched): rows with mask 0 are skipped, their outputs stay
                                  untouched (finished windows of a decode batch); NULL = every row */
@@ -159,8 +159,8 @@ int wts_layernorm(const float* d_x, int64_t ldx, const float* d_gamma, const flo
 int wts_softmax_rows(const float* d_s, int64_t lds, int64_t rows, int32_t n, void* d_out_sb16, int64_t ldo,
                      int64_t o_plane, void* stream);
 
-/* Fused encoder self-attention (tcgen05): out = softmax(q k^T) v per (window, head), head dim 64; the score matrix
- * stays on the SM (TMEM / shared memory).  d_qk: SB16 [B*n_ctx, 2D] (q | k, scale already folded in);
+/* Fused encoder self-attention (wgmma): out = softmax(q k^T) v per (window, head), head dim 64; the score matrix
+ * stays on the SM (registers / shared memory).  d_qk: SB16 [B*n_ctx, 2D] (q | k, scale already folded in);
  * d_vt: SB16 V^T [B*D, ld_vt] (row = channel, column = key); d_out: SB16 [B*n_ctx, D]. */
 int wts_enc_attention(const void* d_qk, int64_t ld_qk, int64_t qk_plane, const void* d_vt, int64_t ld_vt,
                       int64_t vt_plane, int32_t B, int32_t H, int32_t D, int32_t n_ctx, void* d_out, int64_t ldo,
@@ -296,7 +296,7 @@ int wts_decode_steps(const WtsDecodeSteps* p, void* stream);
 
 /* The same step as a chain of per-phase kernels under programmatic dependent launch (2 + 8 n_layer + 1 launches; meant to
  * be captured in a CUDA graph and replayed once per token): a kernel boundary costs less than a software grid barrier
- * across the B200's two dies, and each kernel pulls its weight rows into L2 while its producer drains.  h_layers: HOST
+ * across all SMs, and each kernel pulls its weight rows into L2 while its producer drains.  h_layers: HOST
  * copy of the layer table p->layers points to.  p->max_rows (1..32) sizes the grids and picks the rows-per-pass variant. */
 int wts_decode_step_kernels(const WtsDecodeSteps* p, const WtsDecLayer* h_layers, void* stream);
 

@@ -20,7 +20,7 @@ def _build_everything():
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with -m gpu)")
     _build_everything()
 
 
@@ -30,7 +30,7 @@ def pytest_collection_modifyitems(config, items):
     import torch
     if torch.cuda.is_available():
         return
-    skip = pytest.mark.skip(reason="needs a CUDA device (run on the B200 box: pytest -m gpu)")
+    skip = pytest.mark.skip(reason="needs a CUDA device (run on an H100: pytest -m gpu)")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

@@ -1,4 +1,4 @@
-"""GPU parity tests proper for the alignment numerics (run with -m gpu on a B200).
+"""GPU parity tests proper for the alignment numerics (run with -m gpu on an H100).
 
 All calls go through the C-ABI (libwts.so via ctypes); the oracle is only the checker.
 Bars: DTW jumps / paths bit-exact; attention post-processing within 1e-6 absolute of the

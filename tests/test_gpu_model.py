@@ -69,7 +69,7 @@ def test_gemm_backends_vs_torch(backend):
 
 @pytest.mark.parametrize("backend", BACKENDS)
 def test_gemm_skinny_inplace_residual(backend):
-    """Decode-time shape: one M tile, x += A W^T + b in place (tensor-core path: gemm_skinny_kernel, K split over a
+    """Decode-time shape: one M tile, x += A W^T + b in place (tensor-core path: gemm_tc_kernel, K split over a
     thread-block cluster and reduced through distributed shared memory)."""
     from whisper_timestamped.model import SB16
     from whisper_timestamped.engine import CudaEngine
@@ -201,7 +201,7 @@ def test_cross_attention_f16_vs_torch():
 
 
 def test_enc_attention_fused_vs_torch():
-    """wts_enc_attention (tcgen05, scores on-chip) against float64 softmax(q k^T) v of the same SB16 values."""
+    """wts_enc_attention (wgmma, scores on-chip) against float64 softmax(q k^T) v of the same SB16 values."""
     from whisper_timestamped import _native as nat
     from whisper_timestamped.model import SB16
     dev = torch.device("cuda:0")

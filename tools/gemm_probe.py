@@ -1,8 +1,5 @@
-"""GEMM probe.  Times wts_gemm shapes with the kernels' debug modes (WTS_GEMM_DEBUG) to separate launch, prologue,
-operand feed and tensor-pipe time.  Decode shapes are timed as a CUDA graph of dependent launches (what the decode
-step does), so host launch cost does not pollute them.  Results in debug modes are garbage by design.
-  big kernel:    1 = TMA only, 2 = MMA only, 3 = hi*hi only
-  skinny kernel: 1 = TMA only, 2 = MMA only, 4 = no main loop (prologue + epilogue), 5 = launch + exit"""
+"""GEMM probe.  Times wts_gemm on the encoder shapes and on the decode shapes.  Decode shapes are timed as a CUDA graph
+of dependent launches (what the decode step does), so host launch cost does not pollute them."""
 import os
 import sys
 
@@ -25,22 +22,18 @@ def main():
             a.t.normal_()
             b.t.normal_()
             out = SB16(M, N, dev)
-            for mode in (0, 1, 2, 3):
-                os.environ["WTS_GEMM_DEBUG"] = str(mode)
-                for _ in range(3):
-                    eng.gemm(a, b, M, N, K, out_sb=out)
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                reps = 20
-                torch.cuda.synchronize()
-                e0.record()
-                for _ in range(reps):
-                    eng.gemm(a, b, M, N, K, out_sb=out)
-                e1.record()
-                torch.cuda.synchronize()
-                ms = e0.elapsed_time(e1) / reps
-                ktiles = ((M + 127) // 128) * ((N + 127) // 128) * ((K + 63) // 64)
-                print(f"{name:8s} M={M} N={N} K={K} mode={mode}: {ms * 1e3:9.1f} us  {2.0 * M * N * K / ms / 1e9:8.1f} TF/s(alg)  "
-                      f"{ms * 1e-3 * 1.965e9 * 148 / ktiles:7.0f} clk per k-tile per SM", flush=True)
+            for _ in range(3):
+                eng.gemm(a, b, M, N, K, out_sb=out)
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            reps = 20
+            torch.cuda.synchronize()
+            e0.record()
+            for _ in range(reps):
+                eng.gemm(a, b, M, N, K, out_sb=out)
+            e1.record()
+            torch.cuda.synchronize()
+            ms = e0.elapsed_time(e1) / reps
+            print(f"{name:8s} M={M} N={N} K={K}: {ms * 1e3:9.1f} us  {2.0 * M * N * K / ms / 1e9:8.1f} TF/s(alg)", flush=True)
     if which in ("all", "skinny"):
         n_w = 24                      # distinct weight sets so the chain streams weights from HBM like the decode step
         for (M, N, K, name) in [(128, 1280, 1280, "dec out"), (128, 3840, 1280, "dec qkv"), (128, 5120, 1280, "dec fc1"),
@@ -53,37 +46,34 @@ def main():
             bias = torch.zeros(N, device=dev)
             x = torch.zeros(M, N, device=dev)
             out = SB16(M, N, dev)
-            for mode in (0, 1, 2, 4, 5):
-                os.environ["WTS_GEMM_DEBUG"] = str(mode)
 
-                def chain():
-                    for w in ws:
-                        if N == K:
-                            eng.gemm(a, w, M, N, K, bias=bias, residual=x, ldr=N, out_f32=x, ldc=N)
-                        else:
-                            eng.gemm(a, w, M, N, K, bias=bias, act=1, out_sb=out)
-                chain()
-                torch.cuda.synchronize()
-                graph = torch.cuda.CUDAGraph()
-                s = torch.cuda.Stream(device=dev)
-                s.wait_stream(torch.cuda.current_stream(dev))
-                with torch.cuda.stream(s):
-                    with torch.cuda.graph(graph, stream=s):
-                        chain()
-                torch.cuda.current_stream(dev).wait_stream(s)
-                for _ in range(3):
-                    graph.replay()
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                torch.cuda.synchronize()
-                e0.record()
-                for _ in range(10):
-                    graph.replay()
-                e1.record()
-                torch.cuda.synchronize()
-                us = e0.elapsed_time(e1) / 10 / n_w * 1e3
-                print(f"{name:11s} M={M} N={N} K={K} mode={mode}: {us:7.2f} us per GEMM in a graph chain "
-                      f"(weights {4.0 * N * K / 1e6:.1f} MB -> {4.0 * N * K / us / 1e6:.2f} TB/s)", flush=True)
-    os.environ["WTS_GEMM_DEBUG"] = "0"
+            def chain():
+                for w in ws:
+                    if N == K:
+                        eng.gemm(a, w, M, N, K, bias=bias, residual=x, ldr=N, out_f32=x, ldc=N)
+                    else:
+                        eng.gemm(a, w, M, N, K, bias=bias, act=1, out_sb=out)
+            chain()
+            torch.cuda.synchronize()
+            graph = torch.cuda.CUDAGraph()
+            s = torch.cuda.Stream(device=dev)
+            s.wait_stream(torch.cuda.current_stream(dev))
+            with torch.cuda.stream(s):
+                with torch.cuda.graph(graph, stream=s):
+                    chain()
+            torch.cuda.current_stream(dev).wait_stream(s)
+            for _ in range(3):
+                graph.replay()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            torch.cuda.synchronize()
+            e0.record()
+            for _ in range(10):
+                graph.replay()
+            e1.record()
+            torch.cuda.synchronize()
+            us = e0.elapsed_time(e1) / 10 / n_w * 1e3
+            print(f"{name:11s} M={M} N={N} K={K}: {us:7.2f} us per GEMM in a graph chain "
+                  f"(weights {4.0 * N * K / 1e6:.1f} MB -> {4.0 * N * K / us / 1e6:.2f} TB/s)", flush=True)
 
 
 if __name__ == "__main__":

@@ -2,7 +2,7 @@
 
 CPU experiment on the oracle stand-in (float32 torch): every Linear / Conv of the chosen group is replaced by an
 emulation of what the tensor cores compute — operands split into bf16 hi + lo planes, products accumulated in float32 —
-with 3 terms (hi*hi + lo*hi + hi*lo: what gemm_tc_persist_kernel does today), 2 terms (activation low part dropped,
+with 3 terms (hi*hi + lo*hi + hi*lo: what gemm_tc_kernel does), 2 terms (activation low part dropped,
 or weight low part dropped) or 1 term (plain bf16).  Reports max |delta| against the float32 forward of: encoder
 output, teacher-forced decoder logits, pre-softmax cross-attention rows of the alignment heads.
 

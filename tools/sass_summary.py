@@ -1,8 +1,8 @@
-"""profiles/sass_summary.txt: per-kernel counts of the SASS mnemonics that prove which hardware path a kernel uses
-(tcgen05 MMA = UTCHMMA, TMA = UTMALDG / UBLKCP, TMEM loads = LDTM, cp.async = LDGSTS, FP64 adds = DADD ...).
+"""Per-kernel counts of the SASS mnemonics that show which hardware path a kernel uses (wgmma = HGMMA, mma.sync =
+HMMA, TMA = UTMALDG / UBLKCP, mbarrier = SYNCS, cp.async = LDGSTS, FP64 adds = DADD ...).
 Runs `cuobjdump -sass` on the in-tree libwts.so (no GPU needed).
 
-    python tools/sass_summary.py > profiles/sass_summary.txt
+    python tools/sass_summary.py
 """
 import collections
 import os
@@ -12,7 +12,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SO = os.path.join(ROOT, "whisper-timestamped_b200", "whisper_timestamped", "libwts.so")
-WATCH = ["UTCHMMA", "UTCBAR", "UTMALDG", "UTMAPF", "UBLKCP", "LDTM", "SYNCS", "LDGSTS", "HMMA", "DADD", "DSETP", "FFMA",
+WATCH = ["HGMMA", "WARPGROUP", "UTMALDG", "UTMAPF", "UBLKCP", "SYNCS", "LDGSTS", "HMMA", "DADD", "DSETP", "FFMA",
          "SHFL", "LDS", "STS", "LDG", "STG", "ATOM", "RED", "BAR", "STL", "LDL"]
 
 
@@ -30,7 +30,7 @@ def main():
             op = m.group(1)
             counts[kern][op] += 1
             total[kern] += 1
-    print(f"# cuobjdump -sass {os.path.relpath(SO, ROOT)} (sm_100a): static instruction counts per kernel")
+    print(f"# cuobjdump -sass {os.path.relpath(SO, ROOT)} (sm_90a): static instruction counts per kernel")
     print("# kernel | total | " + " ".join(WATCH))
     for k, c in counts.items():
         print(f"{k} | {total[k]} | " + " ".join(f"{w}={c[w]}" for w in WATCH if c[w]))

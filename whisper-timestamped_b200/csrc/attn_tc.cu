@@ -1,114 +1,34 @@
-// Fused encoder self-attention on tcgen05 (sm_100a): softmax(Q K^T) V for 1500 x 1500 positions, head dim 64,
+// Fused encoder self-attention on wgmma (sm_90a): softmax(Q K^T) V for 1500 x 1500 positions, head dim 64,
 // without ever writing the score matrix to HBM.  Replaces the upstream MultiHeadAttention.qkv_attention of the
 // AudioEncoder blocks (reached by the reference through model.transcribe, T.py:904).
 //
-// One CTA per (128-query tile, head, window); 576 threads, warp-specialised:
-//   warp 0     TMA producer (Q tile once; K tiles double-buffered; V^T tile per key tile in pass 2)
-//   warp 1     MMA issuer   S = Q K^T (bf16x3, M128 N128 K64) into a double-buffered TMEM score tile,
-//                           O += P V (bf16x3, M128 N64 K128) into a TMEM accumulator
-//   warps 2-17 softmax      FOUR threads per query row (warp w: TMEM lanes 32*(w%4).., the 32-key column part
-//                           (w-2)/4 of every 128-key tile): tcgen05.ld the scores, exp, partial row max / sums
-//                           (merged through shared memory), and the probabilities written back to shared memory
-//                           (hi/lo bf16, SWIZZLE_128B K-major) as the A operand of the second MMA.  The softmax
-//                           side, not the tensor pipe, bounds this kernel: with one warp per scheduler it ran
-//                           latency-bound, four warps per scheduler hide the ALU/MUFU/convert latencies
+// One CTA per (128-query tile, head, window); 288 threads:
+//   warp 8 (one lane)  TMA producer: the Q tile once, then one 128-key K tile per step (pass 1) or one K tile and the
+//                      matching V^T tile (pass 2) into a 2-stage ring
+//   warpgroups 0, 1    queries 64*wg .. 64*wg+63: S = Q K^T (bf16x3, wgmma.m64n128k16, both operands in shared memory)
+//                      into registers; softmax on the accumulator fragment; O += P V (bf16x3, wgmma.m64n64k16) with the
+//                      probabilities as the REGISTER A operand (hi/lo bf16 split of the S fragment, no shared memory)
 // Two passes over the keys instead of an online-softmax rescale: pass 1 finds the exact row maxima (S only),
 // pass 2 recomputes S, accumulates exp(s - max) and P V, and the epilogue divides by the row sum.  The extra
-// Q K^T costs 1/3 more tensor work but no TMEM read-modify-write of O, and the score tile never leaves the SM.
+// Q K^T costs 1/3 more tensor work but no rescaling of O, and the score tile never leaves the SM.
 // Operands are SB16 (hi/lo bf16 planes); scale is folded into the q/k projection weights.
-#include <cuda.h>
 #include <cuda_bf16.h>
-#include <cudaTypedefs.h>
 
-#include <mutex>
-
-#include "common.cuh"
+#include "sm90.cuh"
 
 namespace wts {
 
-constexpr int AT_PARTS = 4;                         // column parts (softmax threads per query row)
-constexpr int AT_THREADS = 64 + 128 * AT_PARTS;
-constexpr int AT_Q = 0, AT_K = 32768, AT_V = 98304, AT_P = 131072, AT_BAR = 196608;
-constexpr int AT_XCH = AT_BAR + 256;                // float [AT_PARTS][128] row max / row sum exchange
-constexpr int AT_SMEM = AT_XCH + AT_PARTS * 512 + 1024;
+constexpr int AT_THREADS = 288;
+constexpr int AT_Q = 0, AT_K = 32768, AT_V = 98304, AT_BAR = 163840;
+constexpr int AT_SMEM = AT_BAR + 256 + 1024;
 // barrier slots (8 bytes each) relative to AT_BAR
-enum { B_QFULL = 0, B_KFULL = 1, B_KEMPTY = 3, B_VFULL = 5, B_VEMPTY = 6, B_SFULL = 7, B_SEMPTY = 9, B_PFULL = 11,
-       B_PEMPTY = 12, B_OFULL = 13, B_TMEM = 14 };
+enum { B_QFULL = 0, B_FULL = 1, B_EMPTY = 3 };
 
-__device__ __forceinline__ uint32_t at_smem(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void at_mbar_init(uint32_t bar, uint32_t count)
-{
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void at_expect_tx(uint32_t bar, uint32_t bytes)
-{
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void at_arrive(uint32_t bar)
-{
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void at_wait(uint32_t bar, uint32_t parity)
-{
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "AT_WAIT:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra AT_DONE;\n\t"
-        "bra AT_WAIT;\n\t"
-        "AT_DONE:\n\t"
-        "}\n" ::"r"(bar), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void at_tma_4d(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1, int c2, int c3)
-{
-    asm volatile(
-        "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-        ::"r"(dst), "l"(tm), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void at_umma(uint32_t tmem_c, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc)
-{
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_c), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ void at_commit(uint32_t bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void at_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void at_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void at_ld32(uint32_t taddr, uint32_t (&v)[32])
-{
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-          "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-          "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void at_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ float at_ex2(float x)
 {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
-}
-__device__ __forceinline__ uint64_t at_desc(uint32_t saddr)      // K-major, SWIZZLE_128B, 8-row groups 1024 B apart
-{
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
 }
 
 struct AttnArgs {
@@ -117,263 +37,170 @@ struct AttnArgs {
     int n_ctx, D, H, n_kt;   // n_kt = key tiles of 128
 };
 
+// S[64 x 128] of this warpgroup's queries against key tile st of the ring (bf16x3)
+__device__ __forceinline__ void scores(float (&s)[64], uint64_t q_hi, uint64_t q_lo, uint32_t k_tile)
+{
+    const uint64_t k_hi = wg_desc(k_tile), k_lo = wg_desc(k_tile + 16384);
+    wg_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const uint64_t adv = (uint64_t)(2 * k);
+        wgmma_ss_n128(s, q_hi + adv, k_hi + adv, k ? 1 : 0);
+        wgmma_ss_n128(s, q_lo + adv, k_hi + adv, 1);
+        wgmma_ss_n128(s, q_hi + adv, k_lo + adv, 1);
+    }
+    wg_commit();
+    wg_wait<0>();
+}
+
 __global__ void __launch_bounds__(AT_THREADS, 1)
 enc_attention_tc_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CUtensorMap tmV, const AttnArgs a)
 {
     extern __shared__ unsigned char smem_raw[];
-    const uint32_t base = (at_smem(smem_raw) + 1023u) & ~1023u;
+    const uint32_t base = (smem_addr(smem_raw) + 1023u) & ~1023u;
     const uint32_t bar = base + AT_BAR;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
     const int q0 = qt * 128;
     const int NT = a.n_kt;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 256) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmQK) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmV) : "memory");
-    }
-    if (warp == 1) {
-        if (lane == 0) {
-            at_mbar_init(bar + 8 * B_QFULL, 1);
-            for (int s = 0; s < 2; ++s) {
-                at_mbar_init(bar + 8 * (B_KFULL + s), 1);
-                at_mbar_init(bar + 8 * (B_KEMPTY + s), 1);
-                at_mbar_init(bar + 8 * (B_SFULL + s), 1);
-                at_mbar_init(bar + 8 * (B_SEMPTY + s), 128 * AT_PARTS);
-            }
-            at_mbar_init(bar + 8 * B_VFULL, 1);
-            at_mbar_init(bar + 8 * B_VEMPTY, 1);
-            at_mbar_init(bar + 8 * B_PFULL, 128 * AT_PARTS);
-            at_mbar_init(bar + 8 * B_PEMPTY, 1);
-            at_mbar_init(bar + 8 * B_OFULL, 1);
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_init(bar + 8 * B_QFULL, 1);
+        for (int s = 0; s < 2; ++s) {
+            mbar_init(bar + 8 * (B_FULL + s), 1);
+            mbar_init(bar + 8 * (B_EMPTY + s), 8);
         }
-        __syncwarp();
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(bar + 8 * B_TMEM), "r"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    at_fence_before();
     __syncthreads();
-    at_fence_after();
-    uint32_t tmem;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem) : "r"(bar + 8 * B_TMEM));
-    const uint32_t tm_S0 = tmem, tm_O = tmem + 256;
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (lane == 0) {
             // Q tile: columns h*64.., rows q0.. of window b
-            at_expect_tx(bar + 8 * B_QFULL, 32768);
-            at_tma_4d(base + AT_Q, &tmQK, bar + 8 * B_QFULL, h * 64, q0, b, 0);
-            at_tma_4d(base + AT_Q + 16384, &tmQK, bar + 8 * B_QFULL, h * 64, q0, b, 1);
+            mbar_expect_tx(bar + 8 * B_QFULL, 32768);
+            tma_load_4d(base + AT_Q, &tmQK, bar + 8 * B_QFULL, h * 64, q0, b, 0);
+            tma_load_4d(base + AT_Q + 16384, &tmQK, bar + 8 * B_QFULL, h * 64, q0, b, 1);
             for (int i = 0; i < 2 * NT; ++i) {
                 const int j = i % NT, st = i & 1, u = i >> 1;
-                at_wait(bar + 8 * (B_KEMPTY + st), (u & 1) ^ 1);
-                const uint32_t kf = bar + 8 * (B_KFULL + st);
-                at_expect_tx(kf, 32768);
-                at_tma_4d(base + AT_K + st * 32768, &tmQK, kf, a.D + h * 64, j * 128, b, 0);
-                at_tma_4d(base + AT_K + st * 32768 + 16384, &tmQK, kf, a.D + h * 64, j * 128, b, 1);
-                if (i >= NT) {
-                    const int jj = i - NT;
-                    at_wait(bar + 8 * B_VEMPTY, (jj & 1) ^ 1);
-                    const uint32_t vf = bar + 8 * B_VFULL;
-                    at_expect_tx(vf, 32768);
+                const bool pass2 = i >= NT;
+                mbar_wait(bar + 8 * (B_EMPTY + st), (u & 1) ^ 1);
+                const uint32_t f = bar + 8 * (B_FULL + st);
+                mbar_expect_tx(f, pass2 ? 65536 : 32768);
+                const uint32_t kt = base + AT_K + st * 32768;
+                tma_load_4d(kt, &tmQK, f, a.D + h * 64, j * 128, b, 0);
+                tma_load_4d(kt + 16384, &tmQK, f, a.D + h * 64, j * 128, b, 1);
+                if (pass2) {
                     // V^T tile: rows h*64.. (channels), columns = keys; two 64-key boxes per plane
-                    at_tma_4d(base + AT_V, &tmV, vf, j * 128, h * 64, b, 0);
-                    at_tma_4d(base + AT_V + 8192, &tmV, vf, j * 128 + 64, h * 64, b, 0);
-                    at_tma_4d(base + AT_V + 16384, &tmV, vf, j * 128, h * 64, b, 1);
-                    at_tma_4d(base + AT_V + 24576, &tmV, vf, j * 128 + 64, h * 64, b, 1);
+                    const uint32_t vt = base + AT_V + st * 32768;
+                    tma_load_4d(vt, &tmV, f, j * 128, h * 64, b, 0);
+                    tma_load_4d(vt + 8192, &tmV, f, j * 128 + 64, h * 64, b, 0);
+                    tma_load_4d(vt + 16384, &tmV, f, j * 128, h * 64, b, 1);
+                    tma_load_4d(vt + 24576, &tmV, f, j * 128 + 64, h * 64, b, 1);
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            const uint32_t idesc_s = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(128 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            const uint32_t idesc_o = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(64 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            const uint64_t q_hi = at_desc(base + AT_Q), q_lo = at_desc(base + AT_Q + 16384);
-            at_wait(bar + 8 * B_QFULL, 0);
-            auto issue_S = [&](int i) {
-                const int st = i & 1, u = i >> 1;
-                at_wait(bar + 8 * (B_KFULL + st), u & 1);
-                at_wait(bar + 8 * (B_SEMPTY + st), (u & 1) ^ 1);
-                at_fence_after();
-                const uint64_t k_hi = at_desc(base + AT_K + st * 32768), k_lo = at_desc(base + AT_K + st * 32768 + 16384);
-                const uint32_t tS = tm_S0 + st * 128;
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    const uint64_t adv = (uint64_t)(2 * k);
-                    at_umma(tS, q_hi + adv, k_hi + adv, idesc_s, k ? 1u : 0u);
-                    at_umma(tS, q_lo + adv, k_hi + adv, idesc_s, 1u);
-                    at_umma(tS, q_hi + adv, k_lo + adv, idesc_s, 1u);
-                }
-                at_commit(bar + 8 * (B_KEMPTY + st));
-                at_commit(bar + 8 * (B_SFULL + st));
-            };
-            for (int i = 0; i < NT; ++i) issue_S(i);                  // pass 1: scores only (row maxima)
-            issue_S(NT);
-            for (int j = 0; j < NT; ++j) {                            // pass 2: scores again + P V
-                if (j + 1 < NT) issue_S(NT + j + 1);
-                at_wait(bar + 8 * B_PFULL, j & 1);
-                at_wait(bar + 8 * B_VFULL, j & 1);
-                at_fence_after();
-#pragma unroll
-                for (int at = 0; at < 2; ++at) {
-                    const uint64_t p_hi = at_desc(base + AT_P + at * 16384), p_lo = at_desc(base + AT_P + 32768 + at * 16384);
-                    const uint64_t v_hi = at_desc(base + AT_V + at * 8192), v_lo = at_desc(base + AT_V + 16384 + at * 8192);
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        const uint64_t adv = (uint64_t)(2 * k);
-                        at_umma(tm_O, p_hi + adv, v_hi + adv, idesc_o, (j | at | k) ? 1u : 0u);
-                        at_umma(tm_O, p_lo + adv, v_hi + adv, idesc_o, 1u);
-                        at_umma(tm_O, p_hi + adv, v_lo + adv, idesc_o, 1u);
-                    }
-                }
-                at_commit(bar + 8 * B_PEMPTY);
-                at_commit(bar + 8 * B_VEMPTY);
-            }
-            at_commit(bar + 8 * B_OFULL);
-        }
-    } else {
-        const int q = warp & 3, part = (warp - 2) >> 2;
-        const int r = 32 * q + lane;                    // query row inside the tile == TMEM lane
-        const uint32_t lane_off = (uint32_t)(32 * q) << 16;
-        float* xch = reinterpret_cast<float*>(smem_raw + (base - at_smem(smem_raw)) + AT_XCH);
-        float m = -INFINITY;
-        for (int i = 0; i < NT; ++i) {                  // pass 1: exact row maxima (this thread: 32 of the 128 keys)
-            const int st = i & 1, u = i >> 1;
-            at_wait(bar + 8 * (B_SFULL + st), u & 1);
-            at_fence_after();
-            uint32_t v[32];
-            at_ld32(tm_S0 + st * 128 + lane_off + 32 * part, v);
-            at_ld_wait();
-            at_fence_before();
-            at_arrive(bar + 8 * (B_SEMPTY + st));
-            const int key0 = i * 128 + 32 * part;
-            if (key0 + 32 <= a.n_ctx) {
-                float m0 = __uint_as_float(v[0]), m1 = __uint_as_float(v[1]), m2 = __uint_as_float(v[2]), m3 = __uint_as_float(v[3]);
-#pragma unroll
-                for (int e = 4; e < 32; e += 4) {
-                    m0 = fmaxf(m0, __uint_as_float(v[e]));
-                    m1 = fmaxf(m1, __uint_as_float(v[e + 1]));
-                    m2 = fmaxf(m2, __uint_as_float(v[e + 2]));
-                    m3 = fmaxf(m3, __uint_as_float(v[e + 3]));
-                }
-                m = fmaxf(m, fmaxf(fmaxf(m0, m1), fmaxf(m2, m3)));
-            } else {
-#pragma unroll
-                for (int e = 0; e < 32; ++e)
-                    if (key0 + e < a.n_ctx) m = fmaxf(m, __uint_as_float(v[e]));
-            }
-        }
-        xch[part * 128 + r] = m;
-        asm volatile("bar.sync 1, %0;" ::"n"(128 * AT_PARTS) : "memory");
-#pragma unroll
-        for (int pp = 0; pp < AT_PARTS; ++pp) m = fmaxf(m, xch[pp * 128 + r]);
-        asm volatile("bar.sync 1, %0;" ::"n"(128 * AT_PARTS) : "memory");       // everyone has read before the sums reuse xch
-        float sum = 0.f;
-        const float ml2 = m * 1.4426950408889634f;
-        for (int j = 0; j < NT; ++j) {                  // pass 2: probabilities -> shared memory, partial row sums
-            const int i = NT + j, st = i & 1, u = i >> 1;
-            at_wait(bar + 8 * (B_SFULL + st), u & 1);
-            at_fence_after();
-            uint32_t v[32];
-            at_ld32(tm_S0 + st * 128 + lane_off + 32 * part, v);
-            at_ld_wait();
-            at_fence_before();
-            at_arrive(bar + 8 * (B_SEMPTY + st));       // scores are in registers: the tile can be overwritten
-            const int key0 = j * 128 + 32 * part;
-            const bool tail = key0 + 32 > a.n_ctx;
-            uint32_t hw[16], lw[16];
-            float s0 = 0.f, s1 = 0.f;
-#pragma unroll
-            for (int e = 0; e < 16; ++e) {
-                float p0 = at_ex2(fmaf(__uint_as_float(v[2 * e]), 1.4426950408889634f, -ml2));
-                float p1 = at_ex2(fmaf(__uint_as_float(v[2 * e + 1]), 1.4426950408889634f, -ml2));
-                if (tail) {
-                    if (key0 + 2 * e >= a.n_ctx) p0 = 0.f;
-                    if (key0 + 2 * e + 1 >= a.n_ctx) p1 = 0.f;
-                }
-                s0 += p0;
-                s1 += p1;
-                const __nv_bfloat162 hb = __floats2bfloat162_rn(p0, p1);
-                const uint32_t hbits = *reinterpret_cast<const uint32_t*>(&hb);
-                const float h0 = __uint_as_float(hbits << 16), h1 = __uint_as_float(hbits & 0xffff0000u);
-                const __nv_bfloat162 lb = __floats2bfloat162_rn(p0 - h0, p1 - h1);
-                hw[e] = hbits;
-                lw[e] = *reinterpret_cast<const uint32_t*>(&lb);
-            }
-            sum += s0 + s1;
-            at_wait(bar + 8 * B_PEMPTY, (j & 1) ^ 1);   // previous P V has finished reading the P buffer
-            // A operand of P V: [128 rows x 128 keys] as two 64-key atoms, row pitch 128 B, 16-byte chunks
-            // XOR-swizzled with (row & 7)
-            const uint32_t rowb = base + AT_P + (part >> 1) * 16384 + r * 128;
-#pragma unroll
-            for (int ch = 0; ch < 4; ++ch) {
-                const uint32_t chunk = (uint32_t)((part & 1) * 4 + ch) ^ (uint32_t)(r & 7);
-                asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(rowb + chunk * 16), "r"(hw[4 * ch]), "r"(hw[4 * ch + 1]), "r"(hw[4 * ch + 2]), "r"(hw[4 * ch + 3]) : "memory");
-                asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(rowb + 32768 + chunk * 16), "r"(lw[4 * ch]), "r"(lw[4 * ch + 1]), "r"(lw[4 * ch + 2]), "r"(lw[4 * ch + 3]) : "memory");
-            }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to UMMA
-            at_arrive(bar + 8 * B_PFULL);
-        }
-        xch[part * 128 + r] = sum;
-        asm volatile("bar.sync 1, %0;" ::"n"(128 * AT_PARTS) : "memory");
-        sum = 0.f;
-#pragma unroll
-        for (int pp = 0; pp < AT_PARTS; ++pp) sum += xch[pp * 128 + r];
-        at_wait(bar + 8 * B_OFULL, 0);
-        at_fence_after();
-        const float inv = 1.0f / sum;
-        const int row = q0 + r;
-        if (part < 2) {                                 // the 64 output channels are two 32-column chunks
-            const int c = part;
-            uint32_t v[32];
-            at_ld32(tm_O + lane_off + 32 * c, v);
-            at_ld_wait();
-            if (row < a.n_ctx) {
-                __align__(16) __nv_bfloat16 hi[32];
-                __align__(16) __nv_bfloat16 lo[32];
-#pragma unroll
-                for (int e = 0; e < 32; ++e) {
-                    const float y = __uint_as_float(v[e]) * inv;
-                    hi[e] = __float2bfloat16_rn(y);
-                    lo[e] = __float2bfloat16_rn(y - __bfloat162float(hi[e]));
-                }
-                __nv_bfloat16* dh = a.out + ((int64_t)b * a.n_ctx + row) * a.ldo + h * 64 + 32 * c;
-#pragma unroll
-                for (int ch = 0; ch < 4; ++ch) {
-                    reinterpret_cast<uint4*>(dh)[ch] = reinterpret_cast<const uint4*>(hi)[ch];
-                    reinterpret_cast<uint4*>(dh + a.o_plane)[ch] = reinterpret_cast<const uint4*>(lo)[ch];
-                }
-            }
-        }
+        return;
     }
-    at_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        at_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512) : "memory");
-    }
-}
 
-static PFN_cuTensorMapEncodeTiled_v12000 at_get_encode()
-{
-    static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
-    static std::once_flag once;
-    std::call_once(once, [] {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-            qres == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(p);
-    });
-    return fn;
+    const int wg = warp >> 2;
+    const int cl = 2 * (lane & 3);                  // key / channel column of fragment element 4j: cl + 8j
+    const uint64_t q_hi = wg_desc(base + AT_Q + wg * 8192), q_lo = wg_desc(base + AT_Q + 16384 + wg * 8192);
+    mbar_wait(bar + 8 * B_QFULL, 0);
+    float s[64];
+#pragma unroll
+    for (int e = 0; e < 64; ++e) s[e] = 0.f;
+    // rows r0 = 16*(warp%4) + lane/4 and r0 + 8 of this warpgroup's 64 queries: fragment elements 4j + 0/1 and 4j + 2/3
+    float mx[2] = {-INFINITY, -INFINITY};
+    for (int i = 0; i < NT; ++i) {                  // pass 1: exact row maxima
+        const int st = i & 1, u = i >> 1;
+        mbar_wait(bar + 8 * (B_FULL + st), u & 1);
+        scores(s, q_hi, q_lo, base + AT_K + st * 32768);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar + 8 * (B_EMPTY + st));
+        const int key0 = i * 128 + cl;
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+#pragma unroll
+            for (int e = 0; e < 4; ++e)
+                if (key0 + 8 * j + (e & 1) < a.n_ctx) mx[e >> 1] = fmaxf(mx[e >> 1], s[4 * j + e]);
+    }
+    float ml2[2], sum[2] = {0.f, 0.f};
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        mx[r] = fmaxf(mx[r], __shfl_xor_sync(FULL_MASK, mx[r], 1));
+        mx[r] = fmaxf(mx[r], __shfl_xor_sync(FULL_MASK, mx[r], 2));
+        ml2[r] = mx[r] * 1.4426950408889634f;
+    }
+    float o[32];
+#pragma unroll
+    for (int e = 0; e < 32; ++e) o[e] = 0.f;
+    for (int jt = 0; jt < NT; ++jt) {               // pass 2: probabilities in registers, partial row sums, O += P V
+        const int i = NT + jt, st = i & 1, u = i >> 1;
+        mbar_wait(bar + 8 * (B_FULL + st), u & 1);
+        scores(s, q_hi, q_lo, base + AT_K + st * 32768);
+        const int key0 = jt * 128 + cl;
+        const bool tail = jt * 128 + 128 > a.n_ctx;
+        uint32_t ph[32], pl[32];
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                float p0 = at_ex2(fmaf(s[4 * j + 2 * r], 1.4426950408889634f, -ml2[r]));
+                float p1 = at_ex2(fmaf(s[4 * j + 2 * r + 1], 1.4426950408889634f, -ml2[r]));
+                if (tail) {
+                    if (key0 + 8 * j >= a.n_ctx) p0 = 0.f;
+                    if (key0 + 8 * j + 1 >= a.n_ctx) p1 = 0.f;
+                }
+                sum[r] += p0 + p1;
+                const __nv_bfloat162 hb = __floats2bfloat162_rn(p0, p1);
+                const __nv_bfloat162 lb = __floats2bfloat162_rn(p0 - __low2float(hb), p1 - __high2float(hb));
+                // A fragment of k-step j/2: a0 = (r0, keys 0-7), a1 = (r0+8, keys 0-7), a2 / a3 = the same for keys 8-15
+                const int idx = 4 * (j >> 1) + 2 * (j & 1) + r;
+                ph[idx] = *reinterpret_cast<const uint32_t*>(&hb);
+                pl[idx] = *reinterpret_cast<const uint32_t*>(&lb);
+            }
+        }
+        const uint32_t vt = base + AT_V + st * 32768;
+        wg_fence();
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk) {
+            const uint32_t box = vt + (kk >> 2) * 8192;
+            const uint64_t v_hi = wg_desc(box) + (uint64_t)(2 * (kk & 3)), v_lo = wg_desc(box + 16384) + (uint64_t)(2 * (kk & 3));
+            wgmma_rs_n64(o, ph + 4 * kk, v_hi);
+            wgmma_rs_n64(o, pl + 4 * kk, v_hi);
+            wgmma_rs_n64(o, ph + 4 * kk, v_lo);
+        }
+        wg_commit();
+        wg_wait<0>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar + 8 * (B_EMPTY + st));
+    }
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        sum[r] += __shfl_xor_sync(FULL_MASK, sum[r], 1);
+        sum[r] += __shfl_xor_sync(FULL_MASK, sum[r], 2);
+        const float inv = 1.0f / sum[r];
+        const int row = q0 + 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * r;
+        if (row >= a.n_ctx) continue;
+        __nv_bfloat16* dh = a.out + ((int64_t)b * a.n_ctx + row) * a.ldo + h * 64 + cl;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const float y0 = o[4 * j + 2 * r] * inv, y1 = o[4 * j + 2 * r + 1] * inv;
+            const __nv_bfloat162 hb = __floats2bfloat162_rn(y0, y1);
+            const __nv_bfloat162 lb = __floats2bfloat162_rn(y0 - __low2float(hb), y1 - __high2float(hb));
+            *reinterpret_cast<__nv_bfloat162*>(dh + 8 * j) = hb;
+            *reinterpret_cast<__nv_bfloat162*>(dh + a.o_plane + 8 * j) = lb;
+        }
+    }
 }
 
 // 4-D bf16 map: (cols, rows, batch, plane)
 static int at_make_map(CUtensorMap* tm, const void* ptr, int64_t cols, int64_t rows, int64_t ld, int64_t batch,
                        int64_t batch_stride, int64_t plane, int box_cols, int box_rows, const char* which)
 {
-    auto enc = at_get_encode();
+    auto enc = tensor_map_encoder();
     if (!enc) { set_error("wts_enc_attention: cuTensorMapEncodeTiled entry point not available"); return -4; }
     if ((reinterpret_cast<uintptr_t>(ptr) & 15) || (ld & 7) || (plane & 7) || (batch_stride & 7)) {
         set_error("wts_enc_attention: operand %s not 16-byte aligned", which);
@@ -400,6 +227,10 @@ extern "C" int wts_enc_attention(const void* d_qk, int64_t ld_qk, int64_t qk_pla
 {
     if (B <= 0) return 0;
     if (D != H * 64) { set_error("wts_enc_attention: head dim must be 64 (D=%d H=%d)", D, H); return -2; }
+    if ((reinterpret_cast<uintptr_t>(d_out) & 3) || (ldo & 1) || (o_plane & 1)) {
+        set_error("wts_enc_attention: output not 4-byte aligned");
+        return -5;
+    }
     static bool attr_set = false;
     if (!attr_set) {
         WTS_CUDA_CHECK(cudaFuncSetAttribute(enc_attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AT_SMEM));

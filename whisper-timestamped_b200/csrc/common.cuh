@@ -1,4 +1,4 @@
-// Shared helpers for libwts (sm_100a only).
+// Shared helpers for libwts (sm_90a only).
 #pragma once
 #include <stdlib.h>
 #include <cuda_runtime.h>
@@ -8,8 +8,8 @@
 
 #include "../../include/wts.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libwts is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "libwts is written for sm_90a (H100) only"
 #endif
 
 namespace wts {

@@ -1,16 +1,16 @@
 // Persistent decode-step kernel for SMALL active batches (<= 32 windows still decoding).
 //
 // Why: a decoder step of large-v3 is ~355 dependent kernels when every operator is its own launch; at <= 32 active
-// windows each of them sits at its launch + prologue floor and the step costs ~4 ms against a ~1 ms HBM floor
-// (profiles/r1k_summary.md).  Here ONE cooperative kernel (one CTA per SM, all co-resident) walks
+// windows each of them sits at its launch + prologue floor, far above the time the step's weight stream needs
+// from HBM.  Here ONE cooperative kernel (one CTA per SM, all co-resident) walks
 //     embed -> L x [LN+QKV | self-attn | out-proj | LN+Q | cross-attn | out-proj | LN+FC1+GELU | FC2] -> LN+logits -> select
 // for up to `n_steps` tokens, phases separated by a grid-wide barrier (one atomic + one polling thread per CTA).
 // Replaces, for the whole batch at once, upstream's DecodingTask._main_loop step + the reference's per-token hooks
 // (T.py:783-793 hook_attention_weights, 849-881 hook_output_logits).
 //
 // At <= 32 rows the GEMMs are weight-streaming matrix-vector products, so they run on the FP32 pipe (no tensor cores:
-// a 128-row UMMA tile would be >= 75 % padding and its TMEM/barrier prologue is what made the per-kernel version
-// slow): a warp owns 4 output features, streams their float32 weight rows once (coalesced 512-byte loads, L1
+// a 128-row tensor-core tile would be >= 75 % padding, and its tensor-map/barrier prologue costs a kernel that
+// short more than its math): a warp owns 4 output features, streams their float32 weight rows once (coalesced 512-byte loads, L1
 // bypassed), multiplies them with up to 16 activation rows staged in shared memory (LayerNorm fused into the
 // staging), and reduces over the lanes with a transposing butterfly that leaves every lane with its own outputs.
 // Weights of the NEXT phase are prefetched into L2 before each barrier, so HBM keeps streaming while CTAs wait.
@@ -47,9 +47,8 @@ __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefe
 
 // ---- grid-wide barrier.  Arrivals are one release-add per CTA on a counter; the LAST arriver publishes the new
 // generation on a different 128-byte line, which is the only thing the other CTAs poll (acquire loads with a short
-// back-off) — polls never contend with the arriving atomics (measured: polling the counter itself cost ~6 us per
-// barrier with 148 CTAs; a flag-array barrier — every CTA publishes its generation, warp 0 polls all 148 words — was
-// slower still: ~8 us).  sync[0] = arrivals, sync[1] = error flag, sync[2] = steps completed, sync[32] = generation.
+// back-off) — polls never contend with the arriving atomics (polling the counter itself, or a flag array where every
+// CTA publishes its generation and warp 0 polls all of them, both keep the arrivals waiting on the polls).  sync[0] = arrivals, sync[1] = error flag, sync[2] = steps completed, sync[32] = generation.
 // A spin limit turns a would-be hang (a bug, or a grid that is not co-resident) into an error flag the host reports.
 __device__ __forceinline__ void grid_sync(uint32_t* sync, uint32_t& gen, MgShared& sh)
 {
@@ -315,7 +314,11 @@ __device__ __forceinline__ void prefetch_phase(const float* W, int N, int K, int
     }
 }
 
-constexpr int MG_KV_PREFETCH_ROWS = 8;    // <= 8 rows x 7.7 MB of fp16 K/V per layer stay well inside the 126 MB L2
+// At most this many active rows get their cross-attention K/V prefetched into L2 (a "few rows" step leaves HBM idle
+// during its matrix-vector phases).  The launcher lowers the cap further so that one layer's prefetched fp16 K + V fit
+// in half of the device's L2 (the other half keeps the weight rows the phases stream): large-v3 holds 7.7 MB per row,
+// so a 50 MB L2 takes 3 rows.
+constexpr int MG_KV_PREFETCH_ROWS = 8;
 
 __device__ __forceinline__ void prefetch_cross_kv(const WtsDecodeSteps& P, const WtsDecLayer& Lr, const MgShared& sh)
 {
@@ -435,7 +438,7 @@ __device__ __noinline__ void cross_attention_phase(const WtsDecodeSteps& P, cons
 }
 
 template <int RB>
-__device__ void decode_layers_and_logits(const WtsDecodeSteps& P, MgShared& sh, float* xs, uint32_t& target)
+__device__ void decode_layers_and_logits(const WtsDecodeSteps& P, MgShared& sh, float* xs, uint32_t& target, int kv_pf_rows)
 {
     const int D = P.D, H = P.H;
     const int warp = threadIdx.x >> 5;
@@ -445,7 +448,7 @@ __device__ void decode_layers_and_logits(const WtsDecodeSteps& P, MgShared& sh, 
         const WtsDecLayer& Lr = P.layers[li];
         // few active rows: pull this layer's cross-attention K/V into L2 now (the matrix-vector phases in between leave HBM
         // idle), so the (row, head) streams of P5 — each a single CTA with limited bytes in flight — run at L2 latency
-        if (sh.n_active <= MG_KV_PREFETCH_ROWS) prefetch_cross_kv(P, Lr, sh);
+        if (sh.n_active <= kv_pf_rows) prefetch_cross_kv(P, Lr, sh);
         // P1: LN + QKV
         gemv_phase<RB, true>(Lr.w_qkv, 3 * D, D, D, Lr.b_qkv, P.x, D, Lr.ln1_g, Lr.ln1_b, P.qkv, 3 * D, EPI_STORE, sh, xs);
         prefetch_phase(Lr.w_o, D, D);
@@ -502,7 +505,7 @@ __device__ __noinline__ void select_phase(const WtsDecodeSteps& P, MgShared& sh)
 // (it only shrinks during a launch); more rows than RB simply take several passes.
 template <int RB>
 __global__ void __launch_bounds__(MG_THREADS, 1)
-decode_steps_kernel(const WtsDecodeSteps P)
+decode_steps_kernel(const WtsDecodeSteps P, const int kv_pf_rows)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     MgShared& sh = *reinterpret_cast<MgShared*>(smem_raw);
@@ -553,7 +556,7 @@ decode_steps_kernel(const WtsDecodeSteps P)
         if (step == 0) prefetch_phase(P.layers[0].w_qkv, 3 * D, D);
         grid_sync(P.sync, target, sh);
 
-        decode_layers_and_logits<RB>(P, sh, xs, target);
+        decode_layers_and_logits<RB>(P, sh, xs, target, kv_pf_rows);
 
         // ---- filters + log-softmax + greedy choice: one CTA per active row
         select_phase(P, sh);
@@ -564,9 +567,9 @@ decode_steps_kernel(const WtsDecodeSteps P)
 
 // ------------------------------------------------------------------------------------------------------------------
 // The same step as a chain of LEAN kernels (one per phase), launched with programmatic dependent launch and replayed
-// as one CUDA graph.  Measured on the B200 (tools/step_probe.py, phase timeline): a software grid barrier costs ~5 us
-// (atomics + polling across the two dies' L2) — 259 of them per step put the persistent kernel at ~3.8 ms per step
-// even for one active window.  A kernel boundary under PDL is cheaper, and the next kernel's independent prologue
+// as one CUDA graph.  A software grid barrier costs microseconds (atomics + polling through L2), and the persistent
+// kernel needs 259 of them per step even for one active window (tools/step_probe.py times both variants).  A kernel
+// boundary under PDL is cheaper, and the next kernel's independent prologue
 // (pulling its weight rows into L2) runs while the previous one drains.  Same device code per phase.
 __device__ __forceinline__ void build_row_list(const WtsDecodeSteps& P, MgShared& sh)
 {
@@ -661,8 +664,8 @@ lean_select_kernel(const WtsDecodeSteps P)
 
 // ------------------------------------------------------------------------------------------------------------------
 // Tensor-core variant of the lean matrix-vector phase: mma.sync.m16n8k16 (bf16 in, float32 accumulate) with the same
-// 3-term split-bf16 product as the tcgen05 GEMMs (hi*hi + lo*hi + hi*lo), but none of their per-kernel set-up (no TMEM
-// allocation, no tensor maps, no cluster): at 5..32 active windows the FP32-pipe version above is bound by shared-memory
+// 3-term split-bf16 product as the wgmma GEMMs (hi*hi + lo*hi + hi*lo), but none of their per-kernel set-up (no
+// mbarrier ring, no tensor maps, no cluster): at 5..32 active windows the FP32-pipe version above is bound by shared-memory
 // loads (an LDS.128 per 16 FMAs), this one by the weight stream.
 //  * a CTA owns 8 output features per task; its 8 warps split K; each lane's weight fragment for TWO MMAs is ONE 16-byte
 //    load (8 consecutive k of feature n0 + lane/4, both SB16 planes) — made possible by a PERMUTED k order inside every
@@ -995,13 +998,17 @@ extern "C" int wts_decode_steps(const WtsDecodeSteps* p, void* stream)
     if (P.max_rows > MG_MAXROWS) { set_error("wts_decode_steps: at most %d active rows", MG_MAXROWS); return -2; }
     if (P.n_steps <= 0) return 0;
     cudaStream_t st = (cudaStream_t)stream;
-    static int n_sm = 0;
+    static int n_sm = 0, l2_bytes = 0;
     static size_t smem_set = 0;
     if (n_sm == 0) {
         int dev = 0;
         WTS_CUDA_CHECK(cudaGetDevice(&dev));
         WTS_CUDA_CHECK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
+        WTS_CUDA_CHECK(cudaDeviceGetAttribute(&l2_bytes, cudaDevAttrL2CacheSize, dev));
     }
+    const int64_t kv_row_bytes = 2 * (int64_t)P.H * P.n_audio_ctx * 64 * 2;     // fp16 K + V of one row, one layer
+    int kv_pf_rows = (int)((int64_t)l2_bytes / 2 / kv_row_bytes);
+    if (kv_pf_rows > MG_KV_PREFETCH_ROWS) kv_pf_rows = MG_KV_PREFETCH_ROWS;
     const size_t stage = (size_t)MG_STAGE_FLOATS * sizeof(float);             // gemv_phase sizes its chunks for this capacity
     size_t smem = stage > sizeof(CaScratch) ? stage : sizeof(CaScratch);
     const size_t sa = (size_t)MG_WARPS * P.n_ctx * sizeof(float);             // self-attention score scratch
@@ -1015,7 +1022,7 @@ extern "C" int wts_decode_steps(const WtsDecodeSteps* p, void* stream)
         smem_set = smem;
     }
     WTS_CUDA_CHECK(cudaMemsetAsync(P.sync, 0, 64 * sizeof(uint32_t), st));
-    void* args[] = {const_cast<WtsDecodeSteps*>(p)};
+    void* args[] = {const_cast<WtsDecodeSteps*>(p), &kv_pf_rows};
     const void* fn = P.max_rows <= 4 ? (const void*)decode_steps_kernel<4>
                    : P.max_rows <= 8 ? (const void*)decode_steps_kernel<8> : (const void*)decode_steps_kernel<16>;
     WTS_CUDA_CHECK(cudaLaunchCooperativeKernel(fn, dim3(n_sm), dim3(MG_THREADS), args, smem, st));

@@ -1,4 +1,4 @@
-// Batched monotonic DTW (symmetric1) as a warp-wavefront kernel for sm_100a.
+// Batched monotonic DTW (symmetric1) as a warp-wavefront kernel for sm_90a.
 //
 // Replaces  dtw.dtw(weights, step_pattern=dtw.stepPattern.symmetric1)   (T.py:1572-1581)
 // and the jumps extraction                                              (T.py:1648-1652)
@@ -313,7 +313,7 @@ dtw_warp_kernel(const TIn* __restrict__ cost, const WtsSegDesc* __restrict__ seg
 // The typical alignment problem (T <= 31 tokens, F <= 354 frames, float32 costs <= 0 from wts_attn_prep_batch with rows
 // padded to 16 bytes) gets its own kernel, built to spend as few issue slots per anti-diagonal as the bit-exact fp64
 // recurrence allows (the general kernel above is ISSUE-bound: ~40 warp instructions per step of which the recurrence
-// needs ~17, profiles/r1c_dtw_summary.md):
+// needs ~17):
 //  * staging is 16-byte cp.async (LDGSTS.128): one warp instruction moves 8 rows x 16 columns of a tile, i.e. four
 //    instructions per tile of up to 31 rows, one tile ahead, completion by cp.async groups (rows are padded to 16 bytes
 //    so every chunk is aligned);
@@ -375,8 +375,8 @@ dtw_small_kernel(const float* __restrict__ cost, const WtsSegDesc* __restrict__ 
     const int T = sd.T, F = sd.F, P = (F + 3) & ~3;
     const float* C = cost + sd.cost_off;
     // Optional (WTS_DTW_L2PF=1): one bulk L2 prefetch of the whole contiguous matrix (T x P float32, <= 44 KB), so that
-    // the 64..128-byte tile copies hit L2.  Measured: no effect (0.329 vs 0.323 ms for 16384 matrices) — the kernel is
-    // not bound by the DRAM access pattern.
+    // the 64..128-byte tile copies hit L2.  Off by default: the kernel is bound by its dependent chain, not by the DRAM
+    // access pattern.
     if (lane == 0 && l2_prefetch)
         asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(C), "r"((uint32_t)(T * P * 4)) : "memory");
     // zero the row buffers once: cells read before their tile arrives (j < 0), rows beyond T and the virtual row 0
@@ -928,7 +928,7 @@ extern "C" int wts_dtw_batch_sized(const void* d_cost, int32_t cost_is_f64, cons
             const char* nc_env = getenv("WTS_DTW_LANE_NC");
             const char* g_env = getenv("WTS_DTW_LANE_G");
             const int lane_g = g_env ? atoi(g_env) : 2;
-            const int lane_nc = lane_g == 4 ? 2 : (nc_env && atoi(nc_env) == 2) ? 2 : 4;      // measured: 4 chains with 2 bands
+            const int lane_nc = lane_g == 4 ? 2 : (nc_env && atoi(nc_env) == 2) ? 2 : 4;
 #define WTS_LANE_CASE(TR_)                                                                                                \
             if (lane_rows == TR_) {                                                                                       \
                 if (lane_g == 1)      { if (lane_nc == 2) WTS_LAUNCH_LANE(TR_, 2, 1); else WTS_LAUNCH_LANE(TR_, 4, 1); }  \
@@ -943,7 +943,7 @@ extern "C" int wts_dtw_batch_sized(const void* d_cost, int32_t cost_is_f64, cons
         if (use_small) {
             // geometry variants (WTS_DTW_VARIANT, default 0): <columns per tile, tiles in flight, directions in shared memory>
             static const int variant = [] { const char* e = getenv("WTS_DTW_VARIANT"); return e ? atoi(e) : 4; }();
-            static const int l2pf = [] { const char* e = getenv("WTS_DTW_L2PF"); return e ? atoi(e) : 0; }();   // measured: no effect
+            static const int l2pf = [] { const char* e = getenv("WTS_DTW_L2PF"); return e ? atoi(e) : 0; }();
 #define WTS_LAUNCH_SMALL(TC_, LA_, DS_, IW_)                                                                              \
             do {                                                                                                          \
                 const size_t smem_s = (size_t)n_rows * SmGeo<TC_, LA_>::PITCH * 4 + (DS_ ? n_dir_words * 32 * 4 : 0) + 64;      \
@@ -960,7 +960,7 @@ extern "C" int wts_dtw_batch_sized(const void* d_cost, int32_t cost_is_f64, cons
                 case 4: WTS_LAUNCH_SMALL(32, 1, true, false); break;
                 case 5: WTS_LAUNCH_SMALL(16, 1, false, true); break;
                 case 0: WTS_LAUNCH_SMALL(16, 1, true, false); break;
-                default: WTS_LAUNCH_SMALL(32, 1, true, false); break;        // measured best (DESIGN.md §4.2)
+                default: WTS_LAUNCH_SMALL(32, 1, true, false); break;
             }
 #undef WTS_LAUNCH_SMALL
             WTS_LAUNCH_CHECK();

@@ -1,6 +1,6 @@
 // GEMM of libwts: C = act(alpha * A * B^T + bias) + residual on split-bf16 ("SB16") operands.
 //   backend 1: SIMT float32 kernel (validator / small problems / float32-operand log-mel GEMMs)
-//   backend 0: tcgen05 tensor-core kernel (gemm_tc.cu)
+//   backend 0: wgmma tensor-core kernel (gemm_tc.cu)
 #include <cuda_bf16.h>
 
 #include "common.cuh"

@@ -1,694 +1,249 @@
-// tcgen05 tensor-core GEMM for sm_100a:  C = act(alpha * A * B^T + bias) + residual  on SB16 operands.
+// wgmma tensor-core GEMM for sm_90a:  C = act(alpha * A * B^T + bias) + residual  on SB16 operands.
 //
 // Error-compensated bf16x3: every float32 operand value travels as hi + lo bfloat16 planes and each
-// k-step issues three UMMAs into the same TMEM accumulator:  A_hi*B_hi + A_lo*B_hi + A_hi*B_lo
+// k-step issues three wgmmas into the same register accumulator:  A_hi*B_hi + A_lo*B_hi + A_hi*B_lo
 // (the dropped lo*lo term is ~2^-16 relative).  That keeps logits and cross-attention scores within
-// the 1e-3 bar of the reference's float32 CPU path while running on the 5th-generation tensor cores.
+// the 1e-3 bar of the reference's float32 CPU path while running on the tensor cores.
 //
-// gemm_tc_kernel: one CTA per 128x128 output tile, 192 threads, warp-specialised:
-//   warp 0 (one lane)  TMA producer: 4 boxes (A_hi, A_lo, B_hi, B_lo; 64 x 128 bf16, SWIZZLE_128B) per
-//                      k-block into a 3-stage shared-memory ring, completion on an mbarrier (expect_tx)
-//   warp 1 (one lane)  MMA issuer: tcgen05.mma.cta_group::1.kind::f16 M128 N128 K16, accumulator in TMEM
-//                      (128 lanes x 128 fp32 columns); tcgen05.commit releases ring slots / signals the epilogue
-//   warps 2..5         epilogue: tcgen05.ld (32 lanes x 32 columns per warp) -> alpha/bias/GELU/residual ->
-//                      float32 and/or SB16 stores (optionally head-major for the K/V caches)
+// gemm_tc_kernel: one CTA per 128 x 128 output tile, 288 threads:
+//   warpgroups 0, 1   consumers: rows 64*wg .. 64*wg+63 of the tile, wgmma.m64n128k16 from shared memory into a
+//                     64-float register accumulator per thread; the epilogue runs straight from those registers
+//   warp 8 (one lane) TMA producer: 4 boxes (A_hi, A_lo, B_hi, B_lo; 64 x 128 bf16, SWIZZLE_128B) per k-block into a
+//                     3-stage ring; full[s] completes on the byte count, empty[s] once the 8 consumer warps have
+//                     retired the k-block's wgmmas
 // Batched problems (two batch levels) are extra tensor-map dimensions; M/N/K tails rely on TMA zero fill.
 //
-// gemm_skinny_kernel: the decode-time GEMM (M <= 128 rows, one per decoded window), see its own header below.
-#include <cuda.h>
+// Decode-time GEMMs (M <= 128 rows, one per decoded window) are weight-bandwidth bound, and with one CTA per
+// 128-column tile too few SMs would stream the weights.  There K is split over the CTAs of a thread-block CLUSTER
+// (grid z = S, cluster = (1, 1, S), S <= 8): each CTA parks its float32 partial tile in its own shared memory (the
+// idle operand ring), the cluster synchronises, and CTA r reduces rows r, r + S, ... of all S partials over
+// distributed shared memory (ld.shared::cluster) and applies the epilogue to them: no atomics, no global workspace,
+// a fixed summation order (bit-reproducible), and the epilogue itself is spread over S SMs.
 #include <cuda_bf16.h>
-#include <cudaTypedefs.h>
 
-#include <mutex>
 #include <stdlib.h>
 
-#include "common.cuh"
+#include "sm90.cuh"
 
 namespace wts {
 
-constexpr int BM = 128, BK = 64;
-constexpr int TILE_BYTES = BM * BK * 2;                 // 16 KB: one 128 x 64 bf16 box (A planes)
-constexpr int TC_THREADS = 192;
-template <int BN> struct TcCfg {
-    static constexpr int STAGES = 3;
-    static constexpr int B_TILE = BN * BK * 2;
-    static constexpr int STAGE_BYTES = 2 * TILE_BYTES + 2 * B_TILE;
-    static constexpr int SMEM = STAGES * STAGE_BYTES + 256 + 1024;
-    static constexpr int TMEM_COLS = BN < 32 ? 32 : BN;
-};
-
-// ---------------------------------------------------------------------------------------------- PTX
-__device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count)
-{
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes)
-{
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity)
-{
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "WAIT_LOOP:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra DONE;\n\t"
-        "bra WAIT_LOOP;\n\t"
-        "DONE:\n\t"
-        "}\n" ::"r"(bar), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1, int c2,
-                                            int c3, int c4)
-{
-    asm volatile(
-        "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-        ::"r"(dst), "l"(tm), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_c, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_c), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32])
-{
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-          "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-          "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr) : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// UMMA shared-memory descriptor: K-major, SWIZZLE_128B, 8-row groups 1024 B apart
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr)
-{
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-    d |= (uint64_t)1 << 16;                       // leading byte offset (unused for swizzled K-major)
-    d |= (uint64_t)(1024 >> 4) << 32;             // stride byte offset
-    d |= (uint64_t)1 << 46;                       // descriptor version (sm_100)
-    d |= (uint64_t)2 << 61;                       // SWIZZLE_128B
-    return d;
-}
+constexpr int BM = 128, BN = 128, BK = 64;
+constexpr int TILE_BYTES = BM * BK * 2;                 // 16 KB: one 128 x 64 bf16 box
+constexpr int STAGES = 3;
+constexpr int STAGE_BYTES = 4 * TILE_BYTES;
+constexpr int GT_THREADS = 288;
+constexpr int GT_SMEM = STAGES * STAGE_BYTES + 256 + 1024;
+constexpr int PART_LD = BN + 4;                         // float pitch of a parked partial tile
+static_assert(BM * PART_LD * 4 <= STAGES * STAGE_BYTES, "the partial tile lives in the operand ring");
 
 __device__ __forceinline__ float gelu_erf_tc(float v) { return 0.5f * v * (1.0f + erff(v * 0.70710678118654752440f)); }
 
 struct TcArgs {
     WtsGemm g;
     int a_has_bo, a_has_bi, b_has_bo, b_has_bi;   // 0 => that batch stride is 0 (operand shared): coordinate 0
-    int debug;                                    // probes (WTS_GEMM_DEBUG): 1 = TMA only, 2 = MMA only, 3 = hi*hi only
+    int split_k;                                  // CTAs of a cluster that share one output tile (1 = no split)
 };
 
-// alpha/bias/GELU/residual + float32 and/or SB16 stores of 32 consecutive columns of one output row
-__device__ __forceinline__ void epilogue_chunk(const WtsGemm& g, float (&y)[32], int m, int nb, float bias_m, const float* res,
-                                               float* of, __nv_bfloat16* ob)
+__device__ __forceinline__ int64_t out_offset(const WtsGemm& g, int m, int n, int64_t ld)
 {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-        const int n = nb + j;
-        float t = y[j];
-        if (g.bias) t += g.bias_on_m ? bias_m : (n < g.N ? g.bias[n] : 0.f);
-        if (g.act == 1) t = gelu_erf_tc(t);
-        if (res && n < g.N) t += res[n];
-        y[j] = t;
+    return g.head_dim > 0 ? (int64_t)(n / g.head_dim) * g.head_stride + (int64_t)m * ld + (n % g.head_dim)
+                          : (int64_t)m * ld + n;
+}
+
+__device__ __forceinline__ void store_one(const WtsGemm& g, int m, int n, float t, float* of, __nv_bfloat16* ob)
+{
+    if (of) of[out_offset(g, m, n, g.ldc)] = t;
+    if (ob) {
+        const __nv_bfloat16 hi = __float2bfloat16_rn(t);
+        __nv_bfloat16* d = ob + out_offset(g, m, n, g.ldo);
+        d[0] = hi;
+        d[g.o_plane] = __float2bfloat16_rn(t - __bfloat162float(hi));
     }
-    const bool full = nb + 32 <= g.N;
+}
+
+// alpha/bias/GELU/residual + float32 and/or SB16 stores of output columns n, n+1 (n even) of row m
+__device__ __forceinline__ void epilogue_pair(const WtsGemm& g, int m, int n, float v0, float v1, float bias_m,
+                                              const float* res, float* of, __nv_bfloat16* ob)
+{
+    const bool two = n + 1 < g.N;
+    float t0 = g.alpha * v0, t1 = g.alpha * v1;
+    if (g.bias) {
+        t0 += g.bias_on_m ? bias_m : g.bias[n];
+        if (two) t1 += g.bias_on_m ? bias_m : g.bias[n + 1];
+    }
+    if (g.act == 1) { t0 = gelu_erf_tc(t0); t1 = gelu_erf_tc(t1); }
+    if (res) { t0 += res[n]; if (two) t1 += res[n + 1]; }
+    const bool same_head = g.head_dim == 0 || (n % g.head_dim) + 1 < g.head_dim;
+    if (!(two && same_head)) {
+        store_one(g, m, n, t0, of, ob);
+        if (two) store_one(g, m, n + 1, t1, of, ob);
+        return;
+    }
     if (of) {
-        const int64_t off = g.head_dim > 0 ? (int64_t)(nb / g.head_dim) * g.head_stride + (int64_t)m * g.ldc + (nb % g.head_dim)
-                                           : (int64_t)m * g.ldc + nb;
-        float* dst = of + off;
-        if (full && ((reinterpret_cast<uintptr_t>(dst) & 15) == 0)) {
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(dst + j) = make_float4(y[j], y[j + 1], y[j + 2], y[j + 3]);
-        } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) if (nb + j < g.N) dst[j] = y[j];
-        }
+        float* d = of + out_offset(g, m, n, g.ldc);
+        if ((reinterpret_cast<uintptr_t>(d) & 7) == 0) *reinterpret_cast<float2*>(d) = make_float2(t0, t1);
+        else { d[0] = t0; d[1] = t1; }
     }
     if (ob) {
-        const int64_t off = g.head_dim > 0 ? (int64_t)(nb / g.head_dim) * g.head_stride + (int64_t)m * g.ldo + (nb % g.head_dim)
-                                           : (int64_t)m * g.ldo + nb;
-        __nv_bfloat16* dh = ob + off;
+        __nv_bfloat16* dh = ob + out_offset(g, m, n, g.ldo);
         __nv_bfloat16* dl = dh + g.o_plane;
-        __align__(16) __nv_bfloat16 hi[32];
-        __align__(16) __nv_bfloat16 lo[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-            hi[j] = __float2bfloat16_rn(y[j]);
-            lo[j] = __float2bfloat16_rn(y[j] - __bfloat162float(hi[j]));
-        }
-        if (full && ((reinterpret_cast<uintptr_t>(dh) & 15) == 0) && ((reinterpret_cast<uintptr_t>(dl) & 15) == 0)) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                reinterpret_cast<uint4*>(dh)[j] = reinterpret_cast<const uint4*>(hi)[j];
-                reinterpret_cast<uint4*>(dl)[j] = reinterpret_cast<const uint4*>(lo)[j];
-            }
+        const __nv_bfloat162 hi = __floats2bfloat162_rn(t0, t1);
+        const __nv_bfloat162 lo = __floats2bfloat162_rn(t0 - __low2float(hi), t1 - __high2float(hi));
+        if (((reinterpret_cast<uintptr_t>(dh) | reinterpret_cast<uintptr_t>(dl)) & 3) == 0) {
+            *reinterpret_cast<__nv_bfloat162*>(dh) = hi;
+            *reinterpret_cast<__nv_bfloat162*>(dl) = lo;
         } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) if (nb + j < g.N) { dh[j] = hi[j]; dl[j] = lo[j]; }
+            dh[0] = hi.x; dh[1] = hi.y; dl[0] = lo.x; dl[1] = lo.y;
         }
     }
 }
 
-template <int BN>
-__global__ void __launch_bounds__(TC_THREADS, 1)
+__global__ void __launch_bounds__(GT_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcArgs args)
 {
-    using Cfg = TcCfg<BN>;
-    constexpr int STAGES = Cfg::STAGES, STAGE_BYTES = Cfg::STAGE_BYTES, B_TILE = Cfg::B_TILE, TMEM_COLS = Cfg::TMEM_COLS;
     extern __shared__ unsigned char smem_raw[];
     const WtsGemm& g = args.g;
     const uint32_t base = (smem_addr(smem_raw) + 1023u) & ~1023u;
-    const uint32_t bar_base = base + STAGES * STAGE_BYTES;
-    // barriers: full[s] at +8s, empty[s] at +64+8s, tmem_full at +128, tmem pointer at +136
+    const uint32_t bar = base + STAGES * STAGE_BYTES;   // full[s] at +8s, empty[s] at +32+8s
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
-    const int z = blockIdx.z, zo = z / g.batch_inner, zi = z - zo * g.batch_inner;
-    const int nkb = (g.K + BK - 1) / BK;
-    constexpr int kb0 = 0;
+    const int n0 = blockIdx.x * BN, m0 = blockIdx.y * BM;
+    const int S = args.split_k;
+    const int z = S > 1 ? 0 : blockIdx.z, zo = z / g.batch_inner, zi = z - zo * g.batch_inner;
+    const int nkb_all = (g.K + BK - 1) / BK;
+    const int part_k = S > 1 ? blockIdx.z : 0;
+    const int kb0 = (int)((int64_t)part_k * nkb_all / S);
+    const int nkb = (int)((int64_t)(part_k + 1) * nkb_all / S) - kb0;
+    pdl_launch();
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 256) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
+        for (int s = 0; s < STAGES; ++s) { mbar_init(bar + 8 * s, 1); mbar_init(bar + 32 + 8 * s, 8); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        if (lane == 0) {
-            for (int s = 0; s < STAGES; ++s) { mbar_init(bar_base + 8 * s, 1); mbar_init(bar_base + 64 + 8 * s, 1); }
-            mbar_init(bar_base + 128, 1);
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        }
-        __syncwarp();
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(bar_base + 136), "r"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    uint32_t tmem_base;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(bar_base + 136));
+    pdl_wait();                                     // everything above overlapped the previous kernel's tail
 
-    if (warp == 0) {
+    float acc[64];
+    if (warp == 8) {
         if (lane == 0) {
             const int azo = args.a_has_bo ? zo : 0, azi = args.a_has_bi ? zi : 0;
             const int bzo = args.b_has_bo ? zo : 0, bzi = args.b_has_bi ? zi : 0;
-            for (int kb = 0; kb < (args.debug == 2 ? 0 : nkb); ++kb) {
+            for (int kb = 0; kb < nkb; ++kb) {
                 const int s = kb % STAGES, u = kb / STAGES;
-                mbar_wait(bar_base + 64 + 8 * s, (u & 1) ^ 1);
-                const uint32_t full = bar_base + 8 * s;
+                mbar_wait(bar + 32 + 8 * s, (u & 1) ^ 1);
+                const uint32_t full = bar + 8 * s;
                 mbar_expect_tx(full, STAGE_BYTES);
                 const uint32_t st = base + s * STAGE_BYTES;
                 const int kc = (kb0 + kb) * BK;
                 tma_load_5d(st, &tmA, full, kc, m0, azi, azo, 0);
                 tma_load_5d(st + TILE_BYTES, &tmA, full, kc, m0, azi, azo, 1);
                 tma_load_5d(st + 2 * TILE_BYTES, &tmB, full, kc, n0, bzi, bzo, 0);
-                tma_load_5d(st + 2 * TILE_BYTES + B_TILE, &tmB, full, kc, n0, bzi, bzo, 1);
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // instruction descriptor: D=f32, A=B=bf16, both K-major, N=128, M=128
-            const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-            for (int kb = 0; kb < nkb; ++kb) {
-                const int s = kb % STAGES, u = kb / STAGES;
-                if (args.debug != 2) mbar_wait(bar_base + 8 * s, u & 1);
-                tc_fence_after();
-                if (args.debug == 1) {
-                    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar_base + 64 + 8 * s) : "memory");
-                    continue;
-                }
-                const uint32_t st = base + s * STAGE_BYTES;
-                const uint64_t a_hi = umma_desc(st), a_lo = umma_desc(st + TILE_BYTES);
-                const uint64_t b_hi = umma_desc(st + 2 * TILE_BYTES), b_lo = umma_desc(st + 2 * TILE_BYTES + B_TILE);
-#pragma unroll
-                for (int k = 0; k < BK / 16; ++k) {
-                    const uint64_t adv = (uint64_t)(k * 2);       // 32 bytes per K=16 step, in 16-byte units
-                    umma_bf16(tmem_base, a_hi + adv, b_hi + adv, idesc, (kb | k) ? 1u : 0u);
-                    if (args.debug == 3) continue;
-                    umma_bf16(tmem_base, a_lo + adv, b_hi + adv, idesc, 1u);
-                    umma_bf16(tmem_base, a_hi + adv, b_lo + adv, idesc, 1u);
-                }
-                umma_commit(bar_base + 64 + 8 * s);                // frees the ring slot when the MMAs retire
-            }
-            umma_commit(bar_base + 128);                           // accumulator complete
-        }
-    } else {
-        // ---------------- epilogue: warp q = warp % 4 owns TMEM lanes 32q .. 32q+31 (rows of the tile)
-        const int q = warp & 3;
-        const int m = m0 + 32 * q + lane;
-        mbar_wait(bar_base + 128, 0);
-        tc_fence_after();
-        const bool row_ok = m < g.M;
-        const float* res = g.residual ? g.residual + (int64_t)zo * g.r_bo + (int64_t)zi * g.r_bi + (int64_t)m * g.ldr : nullptr;
-        float* of = g.out_f32 ? g.out_f32 + (int64_t)zo * g.c_bo + (int64_t)zi * g.c_bi : nullptr;
-        __nv_bfloat16* ob = g.out_sb16 ? reinterpret_cast<__nv_bfloat16*>(g.out_sb16) + (int64_t)zo * g.o_bo + (int64_t)zi * g.o_bi : nullptr;
-        const float bias_m = (g.bias && g.bias_on_m && row_ok) ? g.bias[m] : 0.f;
-#pragma unroll 1
-        for (int c = 0; c < BN / 32; ++c) {
-            uint32_t v[32];
-            tmem_ld32(tmem_base + ((uint32_t)(32 * q) << 16) + (uint32_t)(32 * c), v);
-            const int nb = n0 + 32 * c;
-            if (!row_ok || nb >= g.N) continue;
-            float y[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) y[j] = g.alpha * __uint_as_float(v[j]);
-            epilogue_chunk(g, y, m, nb, bias_m, res, of, ob);
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-    }
-}
-
-// ---------------------------------------------------------------------------------- persistent big GEMM
-// Same tile math as gemm_tc_kernel, but ONE CTA per SM walks a static list of output tiles (tile = blockIdx.x +
-// i * gridDim.x; N fastest so neighbouring CTAs share the A tile in L2) and the accumulator is double-buffered in
-// TMEM (2 x 128 columns): while the eight epilogue warps drain tile i (bias / GELU / residual / SB16 split / stores),
-// the producer and MMA warps are already streaming tile i+1.  The one-tile-per-CTA kernel spends more time in its
-// prologue + epilogue than in its 20-k-block main loop on the encoder shapes; here that time is hidden.
-//   warp 0      TMA producer (ring position continues across tiles)
-//   warp 1      MMA issuer; waits tmem_empty[buf] before reusing an accumulator, commits tmem_full[buf]
-//   warps 2..9  epilogue: warp w reads TMEM lanes 32*(w%4).. and columns 64*((w-2)/4) .. +63 of the tile
-constexpr int P_THREADS = 320;
-constexpr int P_STAGES = 3;
-constexpr int P_STAGE_BYTES = 4 * TILE_BYTES;
-constexpr int P_SMEM = P_STAGES * P_STAGE_BYTES + 256 + 1024;
-
-__global__ void __launch_bounds__(P_THREADS, 1)
-gemm_tc_persist_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcArgs args)
-{
-    extern __shared__ unsigned char smem_raw[];
-    const WtsGemm& g = args.g;
-    const uint32_t base = (smem_addr(smem_raw) + 1023u) & ~1023u;
-    const uint32_t bar_base = base + P_STAGES * P_STAGE_BYTES;
-    // barriers: full[s] +8s, empty[s] +32+8s, tmem_full[b] +64+8b, tmem_empty[b] +80+8b, tmem pointer +96
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int tiles_n = (g.N + BM - 1) / BM, tiles_m = (g.M + BM - 1) / BM;
-    const int n_tiles = tiles_n * tiles_m * g.batch_outer * g.batch_inner;
-    const int nkb = (g.K + BK - 1) / BK;
-
-    if (warp == 0 && lane == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
-    }
-    if (warp == 1) {
-        if (lane == 0) {
-            for (int s = 0; s < P_STAGES; ++s) { mbar_init(bar_base + 8 * s, 1); mbar_init(bar_base + 32 + 8 * s, 1); }
-            for (int b = 0; b < 2; ++b) { mbar_init(bar_base + 64 + 8 * b, 1); mbar_init(bar_base + 80 + 8 * b, 256); }
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        }
-        __syncwarp();
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(bar_base + 96), "r"(256) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    uint32_t tmem_base;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(bar_base + 96));
-
-    if (warp == 0) {
-        if (lane == 0) {
-            int it = 0;
-            for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
-                const int nt = t % tiles_n, mt = (t / tiles_n) % tiles_m, z = t / (tiles_n * tiles_m);
-                const int zo = z / g.batch_inner, zi = z - zo * g.batch_inner;
-                const int azo = args.a_has_bo ? zo : 0, azi = args.a_has_bi ? zi : 0;
-                const int bzo = args.b_has_bo ? zo : 0, bzi = args.b_has_bi ? zi : 0;
-                const int m0 = mt * BM, n0 = nt * BM;
-                for (int kb = 0; kb < nkb; ++kb, ++it) {
-                    const int s = it % P_STAGES, u = it / P_STAGES;
-                    mbar_wait(bar_base + 32 + 8 * s, (u & 1) ^ 1);
-                    const uint32_t full = bar_base + 8 * s;
-                    mbar_expect_tx(full, P_STAGE_BYTES);
-                    const uint32_t st = base + s * P_STAGE_BYTES;
-                    const int kc = kb * BK;
-                    tma_load_5d(st, &tmA, full, kc, m0, azi, azo, 0);
-                    tma_load_5d(st + TILE_BYTES, &tmA, full, kc, m0, azi, azo, 1);
-                    tma_load_5d(st + 2 * TILE_BYTES, &tmB, full, kc, n0, bzi, bzo, 0);
-                    tma_load_5d(st + 3 * TILE_BYTES, &tmB, full, kc, n0, bzi, bzo, 1);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BM >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-            int it = 0, lt = 0;
-            for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ++lt) {
-                const int buf = lt & 1, ut = lt >> 1;
-                mbar_wait(bar_base + 80 + 8 * buf, (ut & 1) ^ 1);       // epilogue has drained this accumulator
-                tc_fence_after();
-                const uint32_t acc = tmem_base + (uint32_t)(buf * BM);
-                for (int kb = 0; kb < nkb; ++kb, ++it) {
-                    const int s = it % P_STAGES, u = it / P_STAGES;
-                    mbar_wait(bar_base + 8 * s, u & 1);
-                    tc_fence_after();
-                    const uint32_t st = base + s * P_STAGE_BYTES;
-                    const uint64_t a_hi = umma_desc(st), a_lo = umma_desc(st + TILE_BYTES);
-                    const uint64_t b_hi = umma_desc(st + 2 * TILE_BYTES), b_lo = umma_desc(st + 3 * TILE_BYTES);
-#pragma unroll
-                    for (int k = 0; k < BK / 16; ++k) {
-                        const uint64_t adv = (uint64_t)(k * 2);
-                        umma_bf16(acc, a_hi + adv, b_hi + adv, idesc, (kb | k) ? 1u : 0u);
-                        umma_bf16(acc, a_lo + adv, b_hi + adv, idesc, 1u);
-                        umma_bf16(acc, a_hi + adv, b_lo + adv, idesc, 1u);
-                    }
-                    umma_commit(bar_base + 32 + 8 * s);
-                }
-                umma_commit(bar_base + 64 + 8 * buf);
+                tma_load_5d(st + 3 * TILE_BYTES, &tmB, full, kc, n0, bzi, bzo, 1);
             }
         }
     } else {
-        const int q = warp & 3, half = (warp - 2) >> 2;
-        int lt = 0;
-        for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ++lt) {
-            const int nt = t % tiles_n, mt = (t / tiles_n) % tiles_m, z = t / (tiles_n * tiles_m);
-            const int zo = z / g.batch_inner, zi = z - zo * g.batch_inner;
-            const int m0 = mt * BM, n0 = nt * BM;
-            const int buf = lt & 1, ut = lt >> 1;
-            const int m = m0 + 32 * q + lane;
-            const bool row_ok = m < g.M;
-            const float* res = g.residual ? g.residual + (int64_t)zo * g.r_bo + (int64_t)zi * g.r_bi + (int64_t)m * g.ldr : nullptr;
+        const int wg = warp >> 2;
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+        for (int kb = 0; kb < nkb; ++kb) {
+            const int s = kb % STAGES, u = kb / STAGES;
+            mbar_wait(bar + 8 * s, u & 1);
+            const uint32_t st = base + s * STAGE_BYTES;
+            const uint64_t a_hi = wg_desc(st + wg * (TILE_BYTES / 2)), a_lo = wg_desc(st + TILE_BYTES + wg * (TILE_BYTES / 2));
+            const uint64_t b_hi = wg_desc(st + 2 * TILE_BYTES), b_lo = wg_desc(st + 3 * TILE_BYTES);
+            wg_fence();
+#pragma unroll
+            for (int k = 0; k < BK / 16; ++k) {
+                const uint64_t adv = (uint64_t)(k * 2);       // 32 bytes per K=16 step, in 16-byte units
+                wgmma_ss_n128(acc, a_hi + adv, b_hi + adv, 1);
+                wgmma_ss_n128(acc, a_lo + adv, b_hi + adv, 1);
+                wgmma_ss_n128(acc, a_hi + adv, b_lo + adv, 1);
+            }
+            wg_commit();
+            wg_wait<1>();                                     // the previous k-block's wgmmas have retired
+            if (kb > 0 && lane == 0) mbar_arrive(bar + 32 + 8 * ((kb - 1) % STAGES));
+        }
+        wg_wait<0>();
+
+        const int rl = 64 * wg + 16 * (warp & 3) + (lane >> 2);   // tile row of acc[4j + 0/1]; acc[4j + 2/3]: rl + 8
+        const int cl = 2 * (lane & 3);                            // tile column of acc[4j]: cl + 8j
+        if (S == 1) {
             float* of = g.out_f32 ? g.out_f32 + (int64_t)zo * g.c_bo + (int64_t)zi * g.c_bi : nullptr;
             __nv_bfloat16* ob = g.out_sb16 ? reinterpret_cast<__nv_bfloat16*>(g.out_sb16) + (int64_t)zo * g.o_bo + (int64_t)zi * g.o_bi : nullptr;
-            const float bias_m = (g.bias && g.bias_on_m && row_ok) ? g.bias[m] : 0.f;
-            mbar_wait(bar_base + 64 + 8 * buf, ut & 1);
-            tc_fence_after();
-            uint32_t v0[32], v1[32];
-            const uint32_t taddr = tmem_base + ((uint32_t)(32 * q) << 16) + (uint32_t)(buf * BM + 64 * half);
-            tmem_ld32(taddr, v0);
-            tmem_ld32(taddr + 32, v1);
-            tc_fence_before();
-            asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar_base + 80 + 8 * buf) : "memory");   // accumulator free
-            if (!row_ok) continue;
-            float y[32];
-            int nb = n0 + 64 * half;
-            if (nb < g.N) {
 #pragma unroll
-                for (int j = 0; j < 32; ++j) y[j] = g.alpha * __uint_as_float(v0[j]);
-                epilogue_chunk(g, y, m, nb, bias_m, res, of, ob);
-            }
-            nb += 32;
-            if (nb < g.N) {
+            for (int i = 0; i < 2; ++i) {
+                const int m = m0 + rl + 8 * i;
+                if (m >= g.M || (g.row_mask && g.row_mask[m] == 0)) continue;
+                const float* res = g.residual ? g.residual + (int64_t)zo * g.r_bo + (int64_t)zi * g.r_bi + (int64_t)m * g.ldr : nullptr;
+                const float bias_m = (g.bias && g.bias_on_m) ? g.bias[m] : 0.f;
 #pragma unroll
-                for (int j = 0; j < 32; ++j) y[j] = g.alpha * __uint_as_float(v1[j]);
-                epilogue_chunk(g, y, m, nb, bias_m, res, of, ob);
-            }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256) : "memory");
-    }
-}
-
-// ------------------------------------------------------------------------------------ skinny (decode) GEMM
-// M <= 128 rows (one row per decoded window): weight-bandwidth / latency bound, never tensor bound.
-//  * The operands trade places: the 128 x 64 WEIGHT box is the UMMA "A" operand (M = 128 output features), the
-//    activation rows are the "B" operand (UMMA N = rows rounded up to 16; a single window costs a 16-row box, not
-//    128), so the accumulator holds C^T: TMEM lane = output feature n, column = row m.  An epilogue thread owns
-//    one feature and walks the rows: every global access of a warp covers 32 consecutive features of one row.
-//  * K is split over the CTAs of a thread-block CLUSTER (grid = (N tiles, S), cluster = (1, S, 1), S <= 8) so
-//    that one wave of tiles x S CTAs streams the weights.  Each CTA parks its float32 partial tile in its own
-//    shared memory (the idle operand ring), the cluster synchronises, and CTA r reduces rows r*M/S.. of all S
-//    partials over distributed shared memory (ld.shared::cluster) and applies the epilogue to them: no atomics,
-//    no global workspace, a fixed summation order (bit-reproducible), and the epilogue itself is spread over S SMs.
-struct SkArgs {
-    WtsGemm g;
-    int split_k;
-    int bn;                 // UMMA N: rows rounded up to a multiple of 16
-    int stages, stage_bytes;
-    int debug;              // probes (WTS_GEMM_DEBUG): 1 = TMA only, 2 = MMA only, 4 = no main loop, 5 = launch + exit
-};
-
-constexpr int SK_SMEM = 3 * 65536 + 256 + 1024 + 1024;     // ring | barriers | active-row list | alignment slack
-
-__device__ __forceinline__ void sk_finish(const WtsGemm& g, float t, float resid, int m, int n, float bias_n, float* of,
-                                          __nv_bfloat16* ob)
-{
-    if (g.bias) t += g.bias_on_m ? g.bias[m] : bias_n;
-    if (g.act == 1) t = gelu_erf_tc(t);
-    t += resid;
-    if (of) of[(int64_t)m * g.ldc + n] = t;
-    if (ob) {
-        const __nv_bfloat16 hi = __float2bfloat16_rn(t);
-        ob[(int64_t)m * g.ldo + n] = hi;
-        ob[(int64_t)m * g.ldo + n + g.o_plane] = __float2bfloat16_rn(t - __bfloat162float(hi));
-    }
-}
-
-__device__ __forceinline__ void cluster_sync_all()
-{
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
-// Cluster reduction of feature n over the active rows list[rank], list[rank + S], ...: batches of RB rows, all
-// RB x S distributed-shared-memory loads (and the residuals) of a batch in flight together; the sum over the S
-// partials keeps a fixed order.
-template <int SMAX, int RB>
-__device__ __forceinline__ void sk_reduce_rows(const WtsGemm& g, const uint32_t (&peer)[8], int S, const int* list, int rank,
-                                               int n_rows, int n, float bias_n, float* of, __nv_bfloat16* ob)
-{
-#pragma unroll 1
-    for (int kb = rank; kb < n_rows; kb += RB * S) {
-        float x[RB][SMAX], r[RB];
-        int mm[RB];
-#pragma unroll
-        for (int i = 0; i < RB; ++i) {
-            const int k = kb + i * S;
-            const bool ok = k < n_rows;
-            const int m = ok ? list[k] : 0;
-            mm[i] = ok ? m : -1;
-            r[i] = (ok && g.residual) ? g.residual[(int64_t)m * g.ldr + n] : 0.f;
-#pragma unroll
-            for (int s = 0; s < SMAX; ++s) {
-                x[i][s] = 0.f;
-                if (s < S && ok)
-                    asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(x[i][s]) : "r"(peer[s] + (uint32_t)(m * BM * 4)));
-            }
-        }
-#pragma unroll
-        for (int i = 0; i < RB; ++i) {
-            if (mm[i] >= 0) {
-                float t = 0.f;
-#pragma unroll
-                for (int s = 0; s < SMAX; ++s) t += x[i][s];
-                sk_finish(g, t, r[i], mm[i], n, bias_n, of, ob);
-            }
-        }
-    }
-}
-
-__global__ void __launch_bounds__(TC_THREADS, 1)
-gemm_skinny_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX, const SkArgs args)
-{
-    extern __shared__ unsigned char smem_raw[];
-    const WtsGemm& g = args.g;
-    const uint32_t base = (smem_addr(smem_raw) + 1023u) & ~1023u;
-    const uint32_t bar_base = base + 3 * 65536;
-    // barriers: full[s] at +8s (s < 8), empty[s] at +64+8s, tmem_full at +128, tmem pointer at +136
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int n0 = blockIdx.x * BM;
-    const int S = args.split_k;
-    const int nkb_all = (g.K + BK - 1) / BK;
-    const int kb0 = (int)((int64_t)blockIdx.y * nkb_all / S);
-    const int kb1 = (int)((int64_t)(blockIdx.y + 1) * nkb_all / S);
-    const int nkb = args.debug == 4 ? 0 : kb1 - kb0;
-    const int STAGES = args.stages, STAGE_BYTES = args.stage_bytes;
-    const int X_TILE = args.bn * BK * 2;
-    pdl_launch();
-    if (args.debug == 5) { pdl_wait(); return; }
-
-    if (warp == 0 && lane == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmW) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmX) : "memory");
-    }
-    if (warp == 1) {
-        if (lane == 0) {
-            for (int s = 0; s < STAGES; ++s) { mbar_init(bar_base + 8 * s, 1); mbar_init(bar_base + 64 + 8 * s, 1); }
-            mbar_init(bar_base + 128, 1);
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        }
-        __syncwarp();
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(bar_base + 136), "r"(128) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    uint32_t tmem_base;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(bar_base + 136));
-    pdl_wait();                                     // everything above overlapped the previous kernel's tail
-
-    // active rows (row_mask): compact list in shared memory; row k of the list is reduced by cluster CTA k % S
-    int* rows_list = reinterpret_cast<int*>(smem_raw + (bar_base - smem_addr(smem_raw)) + 256);   // [128] + count at [128]
-    if (warp >= 2) {
-        const int t = threadIdx.x - 64;
-        const bool act = t < g.M && (g.row_mask == nullptr || g.row_mask[t] != 0);
-        const unsigned bal = __ballot_sync(0xffffffffu, act);
-        int* wcount = rows_list + 132;              // per-warp counts [4]
-        if (lane == 0) wcount[warp - 2] = __popc(bal);
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        int off = 0;
-        for (int w2 = 0; w2 < warp - 2; ++w2) off += wcount[w2];
-        if (act) rows_list[off + __popc(bal & ((1u << lane) - 1u))] = t;
-        if (t == 0) rows_list[128] = wcount[0] + wcount[1] + wcount[2] + wcount[3];
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-    }
-
-    const int q = warp & 3;
-    const int nl = 32 * q + lane;                  // feature of this epilogue thread inside the tile
-    const int n = n0 + nl;
-    const bool n_ok = n < g.N;
-    float* of = g.out_f32;
-    __nv_bfloat16* ob = reinterpret_cast<__nv_bfloat16*>(g.out_sb16);
-
-    if (warp == 0) {
-        if (lane == 0) {
-            for (int kb = 0; kb < (args.debug == 2 ? 0 : nkb); ++kb) {
-                const int s = kb % STAGES, u = kb / STAGES;
-                mbar_wait(bar_base + 64 + 8 * s, (u & 1) ^ 1);
-                const uint32_t full = bar_base + 8 * s;
-                mbar_expect_tx(full, STAGE_BYTES);
-                const uint32_t st = base + s * STAGE_BYTES;
-                const int kc = (kb0 + kb) * BK;
-                tma_load_5d(st, &tmW, full, kc, n0, 0, 0, 0);
-                tma_load_5d(st + TILE_BYTES, &tmW, full, kc, n0, 0, 0, 1);
-                tma_load_5d(st + 2 * TILE_BYTES, &tmX, full, kc, 0, 0, 0, 0);
-                tma_load_5d(st + 2 * TILE_BYTES + X_TILE, &tmX, full, kc, 0, 0, 0, 1);
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(args.bn >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-            for (int kb = 0; kb < nkb; ++kb) {
-                const int s = kb % STAGES, u = kb / STAGES;
-                if (args.debug != 2) mbar_wait(bar_base + 8 * s, u & 1);
-                tc_fence_after();
-                if (args.debug == 1) {
-                    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar_base + 64 + 8 * s) : "memory");
-                    continue;
-                }
-                const uint32_t st = base + s * STAGE_BYTES;
-                const uint64_t w_hi = umma_desc(st), w_lo = umma_desc(st + TILE_BYTES);
-                const uint64_t x_hi = umma_desc(st + 2 * TILE_BYTES), x_lo = umma_desc(st + 2 * TILE_BYTES + X_TILE);
-#pragma unroll
-                for (int k = 0; k < BK / 16; ++k) {
-                    const uint64_t adv = (uint64_t)(k * 2);
-                    umma_bf16(tmem_base, w_hi + adv, x_hi + adv, idesc, (kb | k) ? 1u : 0u);
-                    umma_bf16(tmem_base, w_lo + adv, x_hi + adv, idesc, 1u);
-                    umma_bf16(tmem_base, w_hi + adv, x_lo + adv, idesc, 1u);
-                }
-                umma_commit(bar_base + 64 + 8 * s);
-            }
-            umma_commit(bar_base + 128);
-        }
-    } else {
-        // ---------------- epilogue, part 1: accumulator (lane = feature, column = row) out of TMEM
-        const int nchunk = (g.M + 31) / 32;
-        const float bias_n = (g.bias && !g.bias_on_m && n_ok) ? g.bias[n] : 0.f;
-        mbar_wait(bar_base + 128, 0);
-        tc_fence_after();
-        float* part = reinterpret_cast<float*>(smem_raw + (base - smem_addr(smem_raw)));   // [rows][128] partial sums
-#pragma unroll 1
-        for (int c = 0; c < nchunk; ++c) {
-            uint32_t v[32];
-            tmem_ld32(tmem_base + ((uint32_t)(32 * q) << 16) + (uint32_t)(32 * c), v);
-            if (S == 1) {
-                if (!n_ok) continue;
-                float r[32];
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const int m = 32 * c + j;
-                    r[j] = (g.residual && m < g.M) ? g.residual[(int64_t)m * g.ldr + n] : 0.f;
-                }
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const int m = 32 * c + j;
-                    if (m < g.M && (g.row_mask == nullptr || g.row_mask[m] != 0))
-                        sk_finish(g, g.alpha * __uint_as_float(v[j]), r[j], m, n, bias_n, of, ob);
-                }
-            } else {
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const int m = 32 * c + j;
-                    if (m < g.M) part[m * BM + nl] = g.alpha * __uint_as_float(v[j]);
+                for (int j = 0; j < 16; ++j) {
+                    const int n = n0 + cl + 8 * j;
+                    if (n < g.N) epilogue_pair(g, m, n, acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1], bias_m, res, of, ob);
                 }
             }
+        } else {
+            // the ring is idle once BOTH warpgroups have retired their wgmmas (every TMA write has landed: all full
+            // barriers were waited)
+            asm volatile("bar.sync 1, 256;" ::: "memory");
+            float* part = reinterpret_cast<float*>(smem_raw + (base - smem_addr(smem_raw)));
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+#pragma unroll
+                for (int j = 0; j < 16; ++j)
+                    *reinterpret_cast<float2*>(part + (rl + 8 * i) * PART_LD + cl + 8 * j) =
+                        make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
         }
     }
     if (S > 1) {
-        // ---------------- part 2: cluster-wide reduction over distributed shared memory
         __syncwarp();
         cluster_sync_all();                          // every partial tile is parked and visible cluster-wide
-        if (warp >= 2 && n_ok) {
+        if (threadIdx.x < 256) {
             uint32_t rank;
             asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(rank));
-            const int n_rows = rows_list[128];
-            const float bias_n = (g.bias && !g.bias_on_m) ? g.bias[n] : 0.f;
-            uint32_t peer[8];
+            const int c = threadIdx.x & 127, half = threadIdx.x >> 7;
+            const int n = n0 + c;
+            if (n < g.N) {
+                uint32_t peer[8];
 #pragma unroll
-            for (int s = 0; s < 8; ++s) {
-                peer[s] = 0;
-                if (s < S) asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(peer[s]) : "r"(base + 4u * nl), "r"(s));
+                for (int s = 0; s < 8; ++s) {
+                    peer[s] = 0;
+                    if (s < S) asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(peer[s]) : "r"(base + 4u * c), "r"(s));
+                }
+                const float bias_n = (g.bias && !g.bias_on_m) ? g.bias[n] : 0.f;
+                float* of = g.out_f32;
+                __nv_bfloat16* ob = reinterpret_cast<__nv_bfloat16*>(g.out_sb16);
+#pragma unroll 1
+                for (int m = (int)rank + S * half; m < g.M; m += 2 * S) {
+                    if (g.row_mask && g.row_mask[m] == 0) continue;
+                    float x[8];
+#pragma unroll
+                    for (int s = 0; s < 8; ++s) {
+                        x[s] = 0.f;
+                        if (s < S) asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(x[s]) : "r"(peer[s] + (uint32_t)(m * PART_LD * 4)));
+                    }
+                    float t = 0.f;
+#pragma unroll
+                    for (int s = 0; s < 8; ++s) t += x[s];                 // fixed order; the zeros past S add nothing
+                    t = g.alpha * t + (g.bias ? (g.bias_on_m ? g.bias[m] : bias_n) : 0.f);
+                    if (g.act == 1) t = gelu_erf_tc(t);
+                    if (g.residual) t += g.residual[(int64_t)m * g.ldr + n];
+                    store_one(g, m, n, t, of, ob);
+                }
             }
-            if (S <= 4) sk_reduce_rows<4, 12>(g, peer, S, rows_list, (int)rank, n_rows, n, bias_n, of, ob);
-            else        sk_reduce_rows<8, 6>(g, peer, S, rows_list, (int)rank, n_rows, n, bias_n, of, ob);
         }
         __syncwarp();
         cluster_sync_all();                          // nobody leaves while a peer may still read its partial tile
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(128) : "memory");
-    }
 }
 
 // ---------------------------------------------------------------------------------------- host side
-static PFN_cuTensorMapEncodeTiled_v12000 get_encode()
-{
-    static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
-    static std::once_flag once;
-    std::call_once(once, [] {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-            qres == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(p);
-    });
-    return fn;
-}
-
 // 5-D bf16 map: (K, rows, inner batch, outer batch, plane); strides in ELEMENTS
 static int make_map(CUtensorMap* tm, const void* ptr, int64_t K, int64_t rows, int64_t ld, int64_t plane, int64_t n_bi,
                     int64_t s_bi, int64_t n_bo, int64_t s_bo, int box_rows, const char* which)
 {
-    auto enc = get_encode();
+    auto enc = tensor_map_encoder();
     if (!enc) { set_error("wts_gemm: cuTensorMapEncodeTiled entry point not available"); return -4; }
     if ((reinterpret_cast<uintptr_t>(ptr) & 15) || (ld & 7) || (plane & 7) || (s_bi & 7) || (s_bo & 7)) {
         set_error("wts_gemm(tc): operand %s not 16-byte aligned (ptr=%p ld=%lld plane=%lld bi=%lld bo=%lld)", which, ptr,
@@ -713,13 +268,14 @@ static int make_map(CUtensorMap* tm, const void* ptr, int64_t K, int64_t rows, i
     return 0;
 }
 
-static int launch_big(const WtsGemm& g, cudaStream_t st)
+int gemm_tc_launch(const WtsGemm& g, cudaStream_t st)
 {
-    constexpr int BN = 128;
-    static bool attr_set = false;
-    if (!attr_set) {
-        WTS_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<BN>::SMEM));
-        attr_set = true;
+    static int n_sm = 0;
+    if (n_sm == 0) {
+        WTS_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GT_SMEM));
+        int dev = 0;
+        WTS_CUDA_CHECK(cudaGetDevice(&dev));
+        WTS_CUDA_CHECK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
     }
     alignas(64) CUtensorMap tmA, tmB;
     int rc = make_map(&tmA, g.a, g.K, g.M, g.lda, g.a_plane, g.batch_inner, g.a_bi, g.batch_outer, g.a_bo, BM, "A");
@@ -730,87 +286,41 @@ static int launch_big(const WtsGemm& g, cudaStream_t st)
     args.g = g;
     args.a_has_bo = g.a_bo != 0; args.a_has_bi = g.a_bi != 0;
     args.b_has_bo = g.b_bo != 0; args.b_has_bi = g.b_bi != 0;
-    { const char* e = getenv("WTS_GEMM_DEBUG"); args.debug = e ? atoi(e) : 0; }
-    static const int persist = []{ const char* e = getenv("WTS_GEMM_PERSIST"); return e ? atoi(e) : 1; }();
-    const int64_t n_tiles = (int64_t)((g.N + BN - 1) / BN) * ((g.M + BM - 1) / BM) * g.batch_outer * g.batch_inner;
-    if (persist && args.debug == 0 && n_tiles > 1) {
-        static bool pattr = false;
-        static int n_sm = 148;
-        if (!pattr) {
-            WTS_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_persist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, P_SMEM));
-            int dev = 0;
-            WTS_CUDA_CHECK(cudaGetDevice(&dev));
-            WTS_CUDA_CHECK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
-            pattr = true;
-        }
-        // equal-length tile lists: the smallest CTA count that still needs the same number of rounds
-        const int64_t rounds = (n_tiles + n_sm - 1) / n_sm;
-        const int ctas = (int)((n_tiles + rounds - 1) / rounds);
-        gemm_tc_persist_kernel<<<ctas, P_THREADS, P_SMEM, st>>>(tmA, tmB, args);
-        WTS_LAUNCH_CHECK();
-        return 0;
+    const int tiles_n = (g.N + BN - 1) / BN, tiles_m = (g.M + BM - 1) / BM, nkb = (g.K + BK - 1) / BK;
+    const int batch = g.batch_outer * g.batch_inner;
+    // WTS_SPLITK=0 disables the K split of decode-time GEMMs
+    static const int splitk = []{ const char* e = getenv("WTS_SPLITK"); return e ? atoi(e) : 1; }();
+    const bool skinny = tiles_m == 1 && batch == 1 && g.head_dim == 0;
+    int split = 1;
+    if (skinny && splitk && 2 * tiles_n <= n_sm) {
+        split = n_sm / tiles_n;
+        if (split > 8) split = 8;                     // portable cluster size
+        if (split > nkb) split = nkb;
     }
-    dim3 grid((g.N + BN - 1) / BN, (g.M + BM - 1) / BM, g.batch_outer * g.batch_inner);
-    gemm_tc_kernel<BN><<<grid, TC_THREADS, TcCfg<BN>::SMEM, st>>>(tmA, tmB, args);
-    WTS_LAUNCH_CHECK();
-    return 0;
-}
-
-static int launch_skinny(const WtsGemm& g, cudaStream_t st, int split_k)
-{
-    static bool attr_set = false;
-    if (!attr_set) {
-        WTS_CUDA_CHECK(cudaFuncSetAttribute(gemm_skinny_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SK_SMEM));
-        attr_set = true;
-    }
-    SkArgs args;
-    args.g = g;
-    args.bn = ((g.M + 15) / 16) * 16;
-    args.stage_bytes = 2 * TILE_BYTES + 2 * args.bn * BK * 2;
-    args.stages = (3 * 65536) / args.stage_bytes;
-    if (args.stages > 8) args.stages = 8;
-    args.split_k = split_k;
-    { const char* e = getenv("WTS_GEMM_DEBUG"); args.debug = e ? atoi(e) : 0; }
-    alignas(64) CUtensorMap tmW, tmX;
-    int rc = make_map(&tmW, g.b, g.K, g.N, g.ldb, g.b_plane, 1, 0, 1, 0, BM, "B(weights)");
-    if (rc) return rc;
-    rc = make_map(&tmX, g.a, g.K, g.M, g.lda, g.a_plane, 1, 0, 1, 0, args.bn, "A(rows)");
-    if (rc) return rc;
+    args.split_k = split;
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((g.N + BM - 1) / BM, split_k, 1);
-    cfg.blockDim = dim3(TC_THREADS, 1, 1);
-    cfg.dynamicSmemBytes = SK_SMEM;
+    cfg.gridDim = dim3(tiles_n, tiles_m, split > 1 ? split : batch);
+    cfg.blockDim = dim3(GT_THREADS, 1, 1);
+    cfg.dynamicSmemBytes = GT_SMEM;
     cfg.stream = st;
     cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 1;
-    attr[0].val.clusterDim.y = split_k;
-    attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 2 : 1;
-    WTS_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_skinny_kernel, tmW, tmX, args));
-    return 0;
-}
-
-int gemm_tc_launch(const WtsGemm& g, cudaStream_t st)
-{
-    // WTS_SKINNY_GEMM=0 sends decode-time GEMMs through the generic kernel; WTS_SPLITK=0 disables the K split
-    static const int skinny = []{ const char* e = getenv("WTS_SKINNY_GEMM"); return e ? atoi(e) : 1; }();
-    static const int splitk = []{ const char* e = getenv("WTS_SPLITK"); return e ? atoi(e) : 1; }();
-    if (skinny && g.M <= BM && g.batch_outer * g.batch_inner == 1 && g.head_dim == 0) {
-        const int tiles = (g.N + BM - 1) / BM, nkb = (g.K + BK - 1) / BK;
-        int split = 1;
-        if (splitk && tiles <= 74) {
-            split = 148 / tiles;
-            if (split > 8) split = 8;                 // portable cluster size
-            if (split > nkb) split = nkb;
-            if (split < 1) split = 1;
-        }
-        return launch_skinny(g, st, split);
+    int na = 0;
+    if (split > 1) {
+        attr[na].id = cudaLaunchAttributeClusterDimension;
+        attr[na].val.clusterDim.x = 1;
+        attr[na].val.clusterDim.y = 1;
+        attr[na].val.clusterDim.z = split;
+        ++na;
     }
-    return launch_big(g, st);
+    if (skinny && pdl_enabled()) {
+        attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr[na].val.programmaticStreamSerializationAllowed = 1;
+        ++na;
+    }
+    cfg.attrs = attr;
+    cfg.numAttrs = na;
+    WTS_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel, tmA, tmB, args));
+    return 0;
 }
 
 }  // namespace wts

@@ -452,7 +452,7 @@ __global__ void logprob_gather_kernel(const float* logits, int64_t ldl, int n, c
 
 using namespace wts;
 
-static inline int grid_for(int64_t n, int block, int cap = 148 * 16)
+static inline int grid_for(int64_t n, int block, int cap = 132 * 16)
 {
     int64_t g = (n + block - 1) / block;
     return (int)(g < 1 ? 1 : (g > cap ? cap : g));

@@ -1,4 +1,4 @@
-// Fused attention post-processing for word alignment (sm_100a).
+// Fused attention post-processing for word alignment (sm_90a).
 //
 // Replaces, for a whole batch of segments at once, the per-segment CPU sequence of
 // /root/reference/whisper_timestamped/transcribe.py:

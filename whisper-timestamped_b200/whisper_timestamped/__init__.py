@@ -1,8 +1,8 @@
-"""B200-native drop-in for the hot path of whisper-timestamped.
+"""H100-native drop-in for the hot path of whisper-timestamped.
 
 Same import name and API surface as the reference package
 (/root/reference/whisper_timestamped/__init__.py:1-10): `transcribe`, `transcribe_timestamped`,
-`load_model`, `__version__`.  All device work goes through libwts.so (hand-written sm_100a CUDA
+`load_model`, `__version__`.  All device work goes through libwts.so (hand-written sm_90a CUDA
 behind the C-ABI of include/wts.h); importing this package fails if that library is missing.
 """
 from . import _native  # noqa: F401  (fails loudly when libwts.so is absent)
@@ -11,4 +11,4 @@ from .model_zoo import ModelDimensions  # noqa: F401
 from .transcribe import transcribe_timestamped  # noqa: F401
 from .transcribe import transcribe_timestamped as transcribe  # noqa: F401
 
-__version__ = "1.15.9+b200.r1"
+__version__ = "1.15.9+h100.r1"

@@ -1,6 +1,6 @@
-"""CUDA engine: log-mel, batched encoder, batched greedy decoder and batched alignment on one B200.
+"""CUDA engine: log-mel, batched encoder, batched greedy decoder and batched alignment on one H100.
 
-Everything on the device goes through libwts (hand-written sm_100a kernels behind the C-ABI of
+Everything on the device goes through libwts (hand-written sm_90a kernels behind the C-ABI of
 include/wts.h); PyTorch only owns the buffers and the stream.  Replaces, for whole batches of 30-s
 windows at a time, what the reference drives one window and one token at a time through upstream
 `model.transcribe` and its forward hooks (/root/reference/whisper_timestamped/transcribe.py:887-904):
@@ -50,13 +50,13 @@ class CudaEngine:
         self.launches = 0
         self.use_graph = os.environ.get("WTS_CUDA_GRAPH", "1") != "0"
         # at most this many sequences still decoding -> the small-batch kernels take over (0 = never, at most 32).
-        # Default 8: measured on large-v3 (tools/step_probe.py, DESIGN.md §4.3) the lean kernels with mma.sync phases beat
-        # the tcgen05 graph up to 8 active windows (3.44 / 3.49 / 3.54 ms vs 3.57 / 3.67 / 3.78) and lose at 16 (4.62 vs 3.98)
+        # Default 8: the lean kernels with mma.sync phases stream the weights without the per-GEMM tile set-up, which
+        # pays off at a few active windows; tools/step_probe.py times both sides of the cut-over
         self.small_batch_rows = min(32, int(os.environ.get("WTS_SMALL_BATCH_ROWS", "8")) if small_batch_rows is None
                                     else int(small_batch_rows))
         self.small_batch_steps = 0
         # how the small-batch steps run: "lean" = chain of per-phase kernels replayed as a CUDA graph (default),
-        # "persistent" = one cooperative kernel with software grid barriers (measured slower on B200: ~5 us per barrier)
+        # "persistent" = one cooperative kernel with software grid barriers (slower: a software grid barrier costs microseconds)
         self.small_batch_mode = os.environ.get("WTS_SMALL_BATCH_MODE", "lean")
         # matrix-vector phases of the lean kernels on mma.sync tensor cores (split-bf16, 3 terms) instead of FP32 FMAs
         self.small_batch_mma = os.environ.get("WTS_SMALL_BATCH_MMA", "1") != "0"

@@ -1,4 +1,4 @@
-"""load_model() and the device-resident Whisper weights of the B200 drop-in.
+"""load_model() and the device-resident Whisper weights of the H100 drop-in.
 
 Replaces `load_model` (/root/reference/whisper_timestamped/transcribe.py:2405-2544) for the
 openai-whisper checkpoint format ({"dims": ..., "model_state_dict": ...}; key names as produced by
@@ -56,7 +56,7 @@ class WhisperB200:
 
     def __init__(self, dims: zoo.ModelDimensions, state_dict, device, name=None, alignment_heads=None):
         if not torch.cuda.is_available():
-            raise nat.WtsError("whisper_timestamped (B200 drop-in) needs a CUDA device: there is no CPU fallback")
+            raise nat.WtsError("whisper_timestamped (H100 drop-in) needs a CUDA device: there is no CPU fallback")
         self.dims = dims
         self.name = name
         self.device = torch.device(device if device is not None else "cuda")
@@ -214,7 +214,7 @@ def load_model(name, device=None, backend="openai-whisper", download_root=None, 
     name: an official model name, a path to an openai-whisper `.pt` checkpoint, or `synthetic:<official name>`.
     """
     if backend not in ("openai-whisper", "openai"):
-        raise ValueError(f"backend '{backend}' is not supported by the B200 drop-in (only 'openai-whisper')")
+        raise ValueError(f"backend '{backend}' is not supported by the H100 drop-in (only 'openai-whisper')")
     if isinstance(name, str) and name.startswith("synthetic:"):
         base = name.split(":", 1)[1]
         if base not in zoo.DIMS:

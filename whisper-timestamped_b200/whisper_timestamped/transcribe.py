@@ -162,8 +162,9 @@ def transcribe_timestamped(
       engine: inject a decode/alignment engine (tests); default = the model's CUDA engine.
       continuous_batching: let the engine admit a stream's next window into the running decode batch as soon as its
               previous window finishes, instead of decoding in rounds that wait for their slowest window.  Same
-              results.  Off by default: on the bench workload (20 % of the windows run to the 224-token limit, so do
-              follow-up windows) it measured 1.6 % slower than rounds; it pays when windows end early and unevenly.
+              results.  Off by default: on the bench workload 20 % of the windows run to the 224-token limit and their
+              follow-up windows belong to the chunks that are already the longest, so there is little to gain; it pays
+              when windows end early and unevenly.
     """
     # ---- option checks, as T.py:223-261
     assert refine_whisper_precision >= 0 and refine_whisper_precision / AUDIO_TIME_PER_TOKEN == round(
@@ -188,7 +189,7 @@ def transcribe_timestamped(
         model = load_model(model)
     if use_backend_timestamps:
         raise NotImplementedError("use_backend_timestamps (upstream whisper.timing / HF token timestamps) is not built in "
-                                  "this B200 drop-in")
+                                  "this H100 drop-in")
     if not naive_approach and temperature != 0:
         raise NotImplementedError(
             "a scalar temperature > 0 inside the one-pass strategy (sampling under the attention hooks) is not built; "

@@ -23,7 +23,7 @@ def check_vad_method(method):
             pairs.append(tuple(pair))
         return pairs
     raise NotImplementedError(
-        f"vad={method!r}: only an explicit list of (start, end) speech timestamps is built in the B200 drop-in "
+        f"vad={method!r}: only an explicit list of (start, end) speech timestamps is built in the H100 drop-in "
         "(silero / auditok models are not available offline)")
 
 
