@@ -1,6 +1,7 @@
 """Encoder probe: one AudioEncoder pass over B synthetic 30-s windows (large-v3 by default); prints the CUDA-event
 time, or serves as the target of an ncu launch list:
-  ncu --cache-control none --metrics gpu__time_duration.sum --csv ... python tools/encoder_probe.py --windows 32 --reps 1"""
+  ncu --cache-control none --metrics gpu__time_duration.sum --csv ... python tools/encoder_probe.py --windows 32 --reps 1
+--profile FILE: one more pass under torch.profiler (CUDA activities), its kernel table written to FILE."""
 import argparse
 import os
 import sys
@@ -16,6 +17,7 @@ def main():
     ap.add_argument("--model", default="synthetic:large-v3")
     ap.add_argument("--windows", type=int, default=32)
     ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--profile", default=None)
     args = ap.parse_args()
     import whisper_timestamped as wt
     from whisper_timestamped.engine import CudaEngine
@@ -32,6 +34,15 @@ def main():
     e1.record()
     torch.cuda.synchronize()
     print(f"encode {args.windows} windows: {e0.elapsed_time(e1) / args.reps:.1f} ms  ({e0.elapsed_time(e1) / args.reps / args.windows:.2f} ms/window)")
+    if args.profile:
+        from torch.profiler import ProfilerActivity, profile
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            eng.encode(jobs)
+            torch.cuda.synchronize()
+        table = prof.key_averages().table(sort_by="cuda_time_total", row_limit=20, max_name_column_width=60)
+        with open(args.profile, "w") as f:
+            f.write(table)
+        print(table)
 
 
 if __name__ == "__main__":

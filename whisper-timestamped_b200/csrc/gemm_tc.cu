@@ -5,20 +5,28 @@
 // (the dropped lo*lo term is ~2^-16 relative).  That keeps logits and cross-attention scores within
 // the 1e-3 bar of the reference's float32 CPU path while running on the tensor cores.
 //
-// gemm_tc_kernel: one CTA per 128 x 128 output tile, 288 threads:
-//   warpgroups 0, 1   consumers: rows 64*wg .. 64*wg+63 of the tile, wgmma.m64n128k16 from shared memory into a
-//                     64-float register accumulator per thread; the epilogue runs straight from those registers
-//   warp 8 (one lane) TMA producer: 4 boxes (A_hi, A_lo, B_hi, B_lo; 64 x 128 bf16, SWIZZLE_128B) per k-block into a
-//                     3-stage ring; full[s] completes on the byte count, empty[s] once the 8 consumer warps have
-//                     retired the k-block's wgmmas
-// Batched problems (two batch levels) are extra tensor-map dimensions; M/N/K tails rely on TMA zero fill.
+// Both kernels feed 128 x 128 output tiles from the same operand ring: per k-block the TMA producer lane loads 4 boxes
+// (A_hi, A_lo, B_hi, B_lo; 128 rows x 64 bf16, SWIZZLE_128B) into one of 3 stages; full[s] completes on the byte
+// count, empty[s] once the consumer warps have retired the k-block's wgmmas.  Batched problems (two batch levels) are
+// extra tensor-map dimensions; M/N/K tails rely on TMA zero fill.  Every output element sums the same k-blocks, k16
+// steps and terms (hi*hi, lo*hi, hi*lo) in the same order in both kernels, so they give bit-identical results.
 //
-// Decode-time GEMMs (M <= 128 rows, one per decoded window) are weight-bandwidth bound, and with one CTA per
-// 128-column tile too few SMs would stream the weights.  There K is split over the CTAs of a thread-block CLUSTER
-// (grid z = S, cluster = (1, 1, S), S <= 8): each CTA parks its float32 partial tile in its own shared memory (the
-// idle operand ring), the cluster synchronises, and CTA r reduces rows r, r + S, ... of all S partials over
-// distributed shared memory (ld.shared::cluster) and applies the epilogue to them: no atomics, no global workspace,
-// a fixed summation order (bit-reproducible), and the epilogue itself is spread over S SMs.
+// gemm_tc_kernel (encoder, cross-K/V, prefill: more than one M tile, batched, or head-major output): persistent,
+// warp-specialized, ping-pong.  grid = min(tiles, SMs), 384 threads:
+//   warpgroup 0      producer: one TMA lane (setmaxnreg lowered); walks the CTA's tiles t = blockIdx.x + i * gridDim.x
+//                    in M-grouped raster order and keeps the ring full ACROSS tile boundaries
+//   warpgroups 1, 2  consumers (setmaxnreg raised): consumer c owns the CTA's tiles i = c, c + 2, ...: a whole 128 x 128
+//                    tile, 2 x wgmma.m64n128k16 x 3 terms per k16 step into 128 accumulator registers per thread.  An
+//                    ordered pair of named barriers makes the two main loops alternate, so one consumer's register-
+//                    direct epilogue runs while the other one's main loop holds the tensor cores.
+//
+// gemm_tc_skinny_kernel (decode time: one M tile, unbatched).  One CTA per 128-column tile, 288 threads: warpgroups 0, 1
+// consume rows 64*wg .. 64*wg+63 (one m64n128k16 x 3 terms per k16 step), warp 8 is the TMA lane.  These GEMMs are
+// weight-bandwidth bound, and with one CTA per 128-column tile too few SMs would stream the weights.  So K is split over
+// the CTAs of a thread-block CLUSTER (grid z = S, cluster = (1, 1, S), S <= 8): each CTA parks its float32 partial tile
+// in its own shared memory (the idle operand ring), the cluster synchronises, and CTA r reduces rows r, r + S, ... of
+// all S partials over distributed shared memory (ld.shared::cluster) and applies the epilogue to them: no atomics, no
+// global workspace, a fixed summation order (bit-reproducible), and the epilogue itself is spread over S SMs.
 #include <cuda_bf16.h>
 
 #include <stdlib.h>
@@ -31,7 +39,11 @@ constexpr int BM = 128, BN = 128, BK = 64;
 constexpr int TILE_BYTES = BM * BK * 2;                 // 16 KB: one 128 x 64 bf16 box
 constexpr int STAGES = 3;
 constexpr int STAGE_BYTES = 4 * TILE_BYTES;
-constexpr int GT_THREADS = 288;
+constexpr int GT_THREADS = 288;                         // skinny kernel
+constexpr int PT_THREADS = 384;                         // persistent kernel: producer + 2 consumer warpgroups
+constexpr int PT_PRODUCER_REGS = 40, PT_CONSUMER_REGS = 232;
+static_assert(128 * PT_PRODUCER_REGS + 256 * PT_CONSUMER_REGS <= 65536, "setmaxnreg plan exceeds the register file");
+constexpr int GROUP_M = 8;                              // M tiles per raster group of the persistent scheduler
 constexpr int GT_SMEM = STAGES * STAGE_BYTES + 256 + 1024;
 constexpr int PART_LD = BN + 4;                         // float pitch of a parked partial tile
 static_assert(BM * PART_LD * 4 <= STAGES * STAGE_BYTES, "the partial tile lives in the operand ring");
@@ -42,6 +54,7 @@ struct TcArgs {
     WtsGemm g;
     int a_has_bo, a_has_bi, b_has_bo, b_has_bi;   // 0 => that batch stride is 0 (operand shared): coordinate 0
     int split_k;                                  // CTAs of a cluster that share one output tile (1 = no split)
+    int pair_stores;                              // no row mask; every even column pair is one aligned store in one head
 };
 
 __device__ __forceinline__ int64_t out_offset(const WtsGemm& g, int m, int n, int64_t ld)
@@ -61,11 +74,9 @@ __device__ __forceinline__ void store_one(const WtsGemm& g, int m, int n, float 
     }
 }
 
-// alpha/bias/GELU/residual + float32 and/or SB16 stores of output columns n, n+1 (n even) of row m
-__device__ __forceinline__ void epilogue_pair(const WtsGemm& g, int m, int n, float v0, float v1, float bias_m,
-                                              const float* res, float* of, __nv_bfloat16* ob)
+// alpha/bias/GELU/residual of output columns n, n+1 (n even; n + 1 only if two) of one row
+__device__ __forceinline__ float2 pair_values(const WtsGemm& g, int n, bool two, float v0, float v1, float bias_m, const float* res)
 {
-    const bool two = n + 1 < g.N;
     float t0 = g.alpha * v0, t1 = g.alpha * v1;
     if (g.bias) {
         t0 += g.bias_on_m ? bias_m : g.bias[n];
@@ -73,6 +84,25 @@ __device__ __forceinline__ void epilogue_pair(const WtsGemm& g, int m, int n, fl
     }
     if (g.act == 1) { t0 = gelu_erf_tc(t0); t1 = gelu_erf_tc(t1); }
     if (res) { t0 += res[n]; if (two) t1 += res[n + 1]; }
+    return make_float2(t0, t1);
+}
+
+// SB16 store of an aligned pair
+__device__ __forceinline__ void store_pair_sb16(__nv_bfloat16* dh, int64_t plane, float t0, float t1)
+{
+    const __nv_bfloat162 hi = __floats2bfloat162_rn(t0, t1);
+    const __nv_bfloat162 lo = __floats2bfloat162_rn(t0 - __low2float(hi), t1 - __high2float(hi));
+    *reinterpret_cast<__nv_bfloat162*>(dh) = hi;
+    *reinterpret_cast<__nv_bfloat162*>(dh + plane) = lo;
+}
+
+// alpha/bias/GELU/residual + float32 and/or SB16 stores of output columns n, n+1 (n even) of row m
+__device__ __forceinline__ void epilogue_pair(const WtsGemm& g, int m, int n, float v0, float v1, float bias_m,
+                                              const float* res, float* of, __nv_bfloat16* ob)
+{
+    const bool two = n + 1 < g.N;
+    const float2 t = pair_values(g, n, two, v0, v1, bias_m, res);
+    const float t0 = t.x, t1 = t.y;
     const bool same_head = g.head_dim == 0 || (n % g.head_dim) + 1 < g.head_dim;
     if (!(two && same_head)) {
         store_one(g, m, n, t0, of, ob);
@@ -87,19 +117,174 @@ __device__ __forceinline__ void epilogue_pair(const WtsGemm& g, int m, int n, fl
     if (ob) {
         __nv_bfloat16* dh = ob + out_offset(g, m, n, g.ldo);
         __nv_bfloat16* dl = dh + g.o_plane;
-        const __nv_bfloat162 hi = __floats2bfloat162_rn(t0, t1);
-        const __nv_bfloat162 lo = __floats2bfloat162_rn(t0 - __low2float(hi), t1 - __high2float(hi));
         if (((reinterpret_cast<uintptr_t>(dh) | reinterpret_cast<uintptr_t>(dl)) & 3) == 0) {
-            *reinterpret_cast<__nv_bfloat162*>(dh) = hi;
-            *reinterpret_cast<__nv_bfloat162*>(dl) = lo;
+            store_pair_sb16(dh, g.o_plane, t0, t1);
         } else {
+            const __nv_bfloat162 hi = __floats2bfloat162_rn(t0, t1);
+            const __nv_bfloat162 lo = __floats2bfloat162_rn(t0 - __low2float(hi), t1 - __high2float(hi));
             dh[0] = hi.x; dh[1] = hi.y; dl[0] = lo.x; dl[1] = lo.y;
         }
     }
 }
 
-__global__ void __launch_bounds__(GT_THREADS, 1)
+// epilogue of one m64n128 accumulator fragment (rows m_base + t/4 and m_base + t/4 + 8 of lane t, see wgmma_ss_n128)
+// straight from registers, output tile column origin n0, batch coordinates (zo, zi).  PAIRS: every column pair of the
+// tile is inside N, inside one head and stored aligned (TcArgs::pair_stores and a whole tile): the pair code without
+// the per-element fallbacks, a fraction of the instructions the epilogue has to stream through the instruction cache.
+template <bool PAIRS>
+__device__ __forceinline__ void epilogue_frag64(const WtsGemm& g, int zo, int zi, int m_base, int n0, const float (&acc)[64])
+{
+    const int lane = threadIdx.x & 31;
+    const int cl = 2 * (lane & 3);                    // tile column of acc[4j]: cl + 8j
+    float* of = g.out_f32 ? g.out_f32 + (int64_t)zo * g.c_bo + (int64_t)zi * g.c_bi : nullptr;
+    __nv_bfloat16* ob = g.out_sb16 ? reinterpret_cast<__nv_bfloat16*>(g.out_sb16) + (int64_t)zo * g.o_bo + (int64_t)zi * g.o_bi : nullptr;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        const int m = m_base + (lane >> 2) + 8 * i;
+        if (m >= g.M || (g.row_mask && g.row_mask[m] == 0)) continue;
+        const float* res = g.residual ? g.residual + (int64_t)zo * g.r_bo + (int64_t)zi * g.r_bi + (int64_t)m * g.ldr : nullptr;
+        const float bias_m = (g.bias && g.bias_on_m) ? g.bias[m] : 0.f;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            const int n = n0 + cl + 8 * j;
+            if (PAIRS) {
+                const float2 t = pair_values(g, n, true, acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1], bias_m, res);
+                if (of) *reinterpret_cast<float2*>(of + out_offset(g, m, n, g.ldc)) = t;
+                if (ob) store_pair_sb16(ob + out_offset(g, m, n, g.ldo), g.o_plane, t.x, t.y);
+            } else if (n < g.N) {
+                epilogue_pair(g, m, n, acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1], bias_m, res, of, ob);
+            }
+        }
+    }
+}
+
+__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void named_bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+
+struct TileCoord { int m0, n0, zo, zi; };
+
+// tile t of the persistent schedule: batch-major; inside a batch item, groups of GROUP_M M tiles, M fastest inside a
+// group, so the tiles in flight at one time share a few A row blocks and B column blocks in L2
+__device__ __forceinline__ TileCoord tile_coord(const WtsGemm& g, int t, int tiles_m, int tiles_n)
+{
+    const int per_batch = tiles_m * tiles_n;
+    const int z = t / per_batch;
+    int r = t - z * per_batch;
+    const int span = GROUP_M * tiles_n;
+    const int grp = r / span;
+    const int m_first = grp * GROUP_M;
+    const int gm = min(GROUP_M, tiles_m - m_first);
+    r -= grp * span;
+    TileCoord c;
+    c.m0 = (m_first + r % gm) * BM;
+    c.n0 = (r / gm) * BN;
+    c.zo = z / g.batch_inner;
+    c.zi = z - c.zo * g.batch_inner;
+    return c;
+}
+
+__global__ void __launch_bounds__(PT_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcArgs args)
+{
+    extern __shared__ unsigned char smem_raw[];
+    const WtsGemm& g = args.g;
+    const uint32_t base = (smem_addr(smem_raw) + 1023u) & ~1023u;
+    const uint32_t bar = base + STAGES * STAGE_BYTES;   // full[s] at +8s, empty[s] at +32+8s
+    const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+    const int tiles_n = (g.N + BN - 1) / BN, tiles_m = (g.M + BM - 1) / BM;
+    const int tiles = tiles_m * tiles_n * g.batch_outer * g.batch_inner;
+    const int nkb = (g.K + BK - 1) / BK;
+    pdl_launch();
+
+    if (threadIdx.x == 0) {
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
+        for (int s = 0; s < STAGES; ++s) { mbar_init(bar + 8 * s, 1); mbar_init(bar + 32 + 8 * s, 4); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    pdl_wait();                                     // everything above overlapped the previous kernel's tail
+
+    if (wg == 0) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PT_PRODUCER_REGS));
+        if (warp == 0 && lane == 0) {
+            int p = 0;                              // ring position: k-block p of the CTA's whole tile sequence
+            for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+                const TileCoord tc = tile_coord(g, t, tiles_m, tiles_n);
+                const int azo = args.a_has_bo ? tc.zo : 0, azi = args.a_has_bi ? tc.zi : 0;
+                const int bzo = args.b_has_bo ? tc.zo : 0, bzi = args.b_has_bi ? tc.zi : 0;
+                for (int kb = 0; kb < nkb; ++kb, ++p) {
+                    const int s = p % STAGES, u = p / STAGES;
+                    mbar_wait(bar + 32 + 8 * s, (u & 1) ^ 1);
+                    const uint32_t full = bar + 8 * s;
+                    mbar_expect_tx(full, STAGE_BYTES);
+                    const uint32_t st = base + s * STAGE_BYTES;
+                    const int kc = kb * BK;
+                    tma_load_5d(st, &tmA, full, kc, tc.m0, azi, azo, 0);
+                    tma_load_5d(st + TILE_BYTES, &tmA, full, kc, tc.m0, azi, azo, 1);
+                    tma_load_5d(st + 2 * TILE_BYTES, &tmB, full, kc, tc.n0, bzi, bzo, 0);
+                    tma_load_5d(st + 3 * TILE_BYTES, &tmB, full, kc, tc.n0, bzi, bzo, 1);
+                }
+            }
+        }
+        return;
+    }
+
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(PT_CONSUMER_REGS));
+    const int c = wg - 1;                           // consumer 0 / 1: the CTA's even / odd tiles
+    float acc[2][64];
+    int l = c;                                      // index of the tile in the CTA's sequence
+    for (int t = blockIdx.x + c * gridDim.x; t < tiles; t += 2 * gridDim.x, l += 2) {
+        // named barrier 1 + c: "consumer c may start its main loop", arrived by the other consumer
+        if (l > 0) named_bar_sync(1 + c, 256);
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int i = 0; i < 64; ++i) acc[h][i] = 0.f;
+        int p = l * nkb;
+        for (int kb = 0; kb < nkb; ++kb, ++p) {
+            const int s = p % STAGES;
+            mbar_wait(bar + 8 * s, (p / STAGES) & 1);
+            const uint32_t st = base + s * STAGE_BYTES;
+            const uint64_t a_hi = wg_desc(st), a_lo = wg_desc(st + TILE_BYTES);
+            const uint64_t b_hi = wg_desc(st + 2 * TILE_BYTES), b_lo = wg_desc(st + 3 * TILE_BYTES);
+            constexpr uint64_t a_half = (TILE_BYTES / 2) >> 4;   // rows 64..127 of an A box, in 16-byte units
+            wg_fence();
+#pragma unroll
+            for (int k = 0; k < BK / 16; ++k) {
+                const uint64_t adv = (uint64_t)(k * 2);       // 32 bytes per K=16 step, in 16-byte units
+#pragma unroll
+                for (int h = 0; h < 2; ++h) wgmma_ss_n128(acc[h], a_hi + h * a_half + adv, b_hi + adv, 1);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) wgmma_ss_n128(acc[h], a_lo + h * a_half + adv, b_hi + adv, 1);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) wgmma_ss_n128(acc[h], a_hi + h * a_half + adv, b_lo + adv, 1);
+            }
+            wg_commit();
+            wg_wait<1>();                                     // the previous k-block's wgmmas have retired
+            if (kb > 0 && lane == 0) mbar_arrive(bar + 32 + 8 * ((p - 1) % STAGES));
+        }
+        // every wgmma of this tile is issued: the other consumer's main loop may start (if it has a next tile)
+        if (t + gridDim.x < tiles) named_bar_arrive(2 - c, 256);
+        wg_wait<0>();
+        if (lane == 0) mbar_arrive(bar + 32 + 8 * ((p - 1) % STAGES));
+
+        const TileCoord tc = tile_coord(g, t, tiles_m, tiles_n);
+        const bool pairs = args.pair_stores && tc.n0 + BN <= g.N;
+        // not unrolled over the two halves: one copy of the epilogue code, fed by a register select
+#pragma unroll 1
+        for (int h = 0; h < 2; ++h) {
+            float v[64];
+#pragma unroll
+            for (int i = 0; i < 64; ++i) v[i] = h ? acc[1][i] : acc[0][i];
+            if (pairs) epilogue_frag64<true>(g, tc.zo, tc.zi, tc.m0 + 64 * h + 16 * warp, tc.n0, v);
+            else epilogue_frag64<false>(g, tc.zo, tc.zi, tc.m0 + 64 * h + 16 * warp, tc.n0, v);
+        }
+    }
+}
+
+__global__ void __launch_bounds__(GT_THREADS, 1)
+gemm_tc_skinny_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcArgs args)
 {
     extern __shared__ unsigned char smem_raw[];
     const WtsGemm& g = args.g;
@@ -169,20 +354,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int rl = 64 * wg + 16 * (warp & 3) + (lane >> 2);   // tile row of acc[4j + 0/1]; acc[4j + 2/3]: rl + 8
         const int cl = 2 * (lane & 3);                            // tile column of acc[4j]: cl + 8j
         if (S == 1) {
-            float* of = g.out_f32 ? g.out_f32 + (int64_t)zo * g.c_bo + (int64_t)zi * g.c_bi : nullptr;
-            __nv_bfloat16* ob = g.out_sb16 ? reinterpret_cast<__nv_bfloat16*>(g.out_sb16) + (int64_t)zo * g.o_bo + (int64_t)zi * g.o_bi : nullptr;
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                const int m = m0 + rl + 8 * i;
-                if (m >= g.M || (g.row_mask && g.row_mask[m] == 0)) continue;
-                const float* res = g.residual ? g.residual + (int64_t)zo * g.r_bo + (int64_t)zi * g.r_bi + (int64_t)m * g.ldr : nullptr;
-                const float bias_m = (g.bias && g.bias_on_m) ? g.bias[m] : 0.f;
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const int n = n0 + cl + 8 * j;
-                    if (n < g.N) epilogue_pair(g, m, n, acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1], bias_m, res, of, ob);
-                }
-            }
+            epilogue_frag64<false>(g, zo, zi, m0 + 64 * wg + 16 * (warp & 3), n0, acc);
         } else {
             // the ring is idle once BOTH warpgroups have retired their wgmmas (every TMA write has landed: all full
             // barriers were waited)
@@ -273,6 +445,7 @@ int gemm_tc_launch(const WtsGemm& g, cudaStream_t st)
     static int n_sm = 0;
     if (n_sm == 0) {
         WTS_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GT_SMEM));
+        WTS_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_skinny_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GT_SMEM));
         int dev = 0;
         WTS_CUDA_CHECK(cudaGetDevice(&dev));
         WTS_CUDA_CHECK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
@@ -288,21 +461,37 @@ int gemm_tc_launch(const WtsGemm& g, cudaStream_t st)
     args.b_has_bo = g.b_bo != 0; args.b_has_bi = g.b_bi != 0;
     const int tiles_n = (g.N + BN - 1) / BN, tiles_m = (g.M + BM - 1) / BM, nkb = (g.K + BK - 1) / BK;
     const int batch = g.batch_outer * g.batch_inner;
+    cudaLaunchConfig_t cfg = {};
+    cfg.dynamicSmemBytes = GT_SMEM;
+    cfg.stream = st;
+    const bool skinny = tiles_m == 1 && batch == 1 && g.head_dim == 0;
+    if (!skinny) {
+        const int64_t tiles = (int64_t)tiles_m * tiles_n * batch;
+        if (tiles > INT32_MAX / 2) { set_error("wts_gemm(tc): %lld output tiles are too many", (long long)tiles); return -7; }
+        args.split_k = 1;
+        const bool heads_even = g.head_dim == 0 || (g.head_dim % 2 == 0 && g.head_stride % 2 == 0);
+        const bool of_pairs = !g.out_f32 || ((reinterpret_cast<uintptr_t>(g.out_f32) & 7) == 0 && g.ldc % 2 == 0 &&
+                                             g.c_bo % 2 == 0 && g.c_bi % 2 == 0);
+        const bool ob_pairs = !g.out_sb16 || ((reinterpret_cast<uintptr_t>(g.out_sb16) & 3) == 0 && g.ldo % 2 == 0 &&
+                                              g.o_plane % 2 == 0 && g.o_bo % 2 == 0 && g.o_bi % 2 == 0);
+        args.pair_stores = !g.row_mask && heads_even && of_pairs && ob_pairs;
+        cfg.gridDim = dim3((unsigned)(tiles < n_sm ? tiles : n_sm), 1, 1);
+        cfg.blockDim = dim3(PT_THREADS, 1, 1);
+        WTS_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel, tmA, tmB, args));
+        return 0;
+    }
     // WTS_SPLITK=0 disables the K split of decode-time GEMMs
     static const int splitk = []{ const char* e = getenv("WTS_SPLITK"); return e ? atoi(e) : 1; }();
-    const bool skinny = tiles_m == 1 && batch == 1 && g.head_dim == 0;
     int split = 1;
-    if (skinny && splitk && 2 * tiles_n <= n_sm) {
+    if (splitk && 2 * tiles_n <= n_sm) {
         split = n_sm / tiles_n;
         if (split > 8) split = 8;                     // portable cluster size
         if (split > nkb) split = nkb;
     }
     args.split_k = split;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(tiles_n, tiles_m, split > 1 ? split : batch);
+    args.pair_stores = 0;
+    cfg.gridDim = dim3(tiles_n, 1, split);
     cfg.blockDim = dim3(GT_THREADS, 1, 1);
-    cfg.dynamicSmemBytes = GT_SMEM;
-    cfg.stream = st;
     cudaLaunchAttribute attr[2];
     int na = 0;
     if (split > 1) {
@@ -312,14 +501,14 @@ int gemm_tc_launch(const WtsGemm& g, cudaStream_t st)
         attr[na].val.clusterDim.z = split;
         ++na;
     }
-    if (skinny && pdl_enabled()) {
+    if (pdl_enabled()) {
         attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
         attr[na].val.programmaticStreamSerializationAllowed = 1;
         ++na;
     }
     cfg.attrs = attr;
     cfg.numAttrs = na;
-    WTS_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel, tmA, tmB, args));
+    WTS_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_tc_skinny_kernel, tmA, tmB, args));
     return 0;
 }
 
