@@ -250,54 +250,47 @@ int wts_filtered_logprobs(const float* d_logits, int64_t ldl, const WtsDecodeCfg
                           const uint8_t* d_blank, int32_t* d_tokens, int32_t* d_n_tokens, const int32_t* d_n_prompt,
                           float* d_out, int32_t B, void* stream);
 
-/* ---- Persistent decode steps for small active batches (csrc/decode_steps.cu).
- * One cooperative kernel runs up to n_steps whole decoder steps (embed, all blocks with KV-cache append, causal
- * self-attention, fp16 cross-attention with the alignment heads' pre-softmax rows written into qk_buf, final LayerNorm,
- * tied-embedding logits, logit filters + log-softmax + greedy choice) for the sequences whose done flag is 0 — at most 32.
- * Replaces upstream DecodingTask._main_loop driven through the reference's hooks (T.py:783-793, 849-881), for the whole
- * batch at once.  Weights are float32 [out, in] row-major; q/k projections carry the d_head^-1/4 scale; the self K/V
- * caches, cross K/V caches, token buffers, log-prob rows and qk_buf are the SAME buffers the per-operator path uses, so
- * the two paths can alternate between steps. */
+/* ---- Decoder step for small active batches (csrc/decode_steps.cu).
+ * One whole decoder step (embed, all blocks with KV-cache append, causal self-attention, fp16 cross-attention with the
+ * alignment heads' pre-softmax rows written into qk_buf, final LayerNorm, tied-embedding logits, logit filters +
+ * log-softmax + greedy choice) for the sequences whose done flag is 0 — at most 32.  Replaces upstream
+ * DecodingTask._main_loop driven through the reference's hooks (T.py:783-793, 849-881), for the whole batch at once.
+ * Matrix weights are SB16 planes; q/k projections carry the d_head^-1/4 scale; the self K/V caches, cross K/V caches,
+ * token buffers, log-prob rows and qk_buf are the SAME buffers the per-operator path uses, so the two paths can
+ * alternate between steps. */
 typedef struct WtsDecLayer {
-    const float *ln1_g, *ln1_b, *w_qkv, *b_qkv, *w_o, *b_o;          /* self-attention block */
-    const float *ln2_g, *ln2_b, *w_cq, *b_cq, *w_co, *b_co;          /* cross-attention block (K/V are cached) */
-    const float *ln3_g, *ln3_b, *w_fc1, *b_fc1, *w_fc2, *b_fc2;      /* MLP */
+    const float *ln1_g, *ln1_b, *b_qkv, *b_o;                        /* self-attention block */
+    const float *ln2_g, *ln2_b, *b_cq, *b_co;                        /* cross-attention block (K/V are cached) */
+    const float *ln3_g, *ln3_b, *b_fc1, *b_fc2;                      /* MLP */
     float *self_k, *self_v;                                          /* [cap, H, n_ctx, 64] float32 */
     const void *cross_k16, *cross_v16;                               /* [cap, H, n_audio_ctx, 64] fp16 */
     const float* cross_k_align;                                      /* [cap, n_slots, n_audio_ctx, 64] float32 */
     const int32_t* head_slot;                                        /* [H]: alignment slot of each head or -1 */
-    /* the same six matrices as split-bf16 (SB16) planes [2][out][in] (hi plane at the pointer, lo plane `pl_*` ELEMENTS
-     * further), row pitch = in: operands of the mma.sync variant of the lean kernels (use_mma) */
+    /* the six matrices as split-bf16 (SB16) planes [2][out][in] (hi plane at the pointer, lo plane `pl_*` ELEMENTS
+     * further), row pitch = in */
     const void *sb_qkv, *sb_o, *sb_cq, *sb_co, *sb_fc1, *sb_fc2;
     int64_t pl_qkv, pl_o, pl_cq, pl_co, pl_fc1, pl_fc2;
 } WtsDecLayer;
 
 typedef struct WtsDecodeSteps {
     const WtsDecLayer* layers;                                       /* device array [n_layer] */
-    const float *emb, *pos, *ln_g, *ln_b;                            /* [V, D], [n_ctx, D], final LayerNorm */
+    const float *emb, *pos, *ln_g, *ln_b;                            /* [V, D] float32 (embedding rows), [n_ctx, D], final LayerNorm */
     int32_t *tokens, *n_tokens;
     const int32_t* n_prompt;
     int32_t* done;
     float *logprobs, *full, *last_full, *qk_buf;                     /* full / last_full optional */
     const uint8_t *suppress, *blank;
     float *x, *qkv, *att, *q, *mid, *logits;                         /* scratch: [cap, D], [cap, 3D], [cap, D], [cap, D], [cap, 4D], [cap, V] */
-    uint32_t* sync;                                                  /* [64] (two 128-byte lines): [0] barrier arrivals, [1] error flag, [2] steps completed, [32] barrier generation */
-    uint64_t* prof;                                                  /* optional: %globaltimer of CTA 0 after every grid barrier */
-    const void* emb_sb;                                              /* token embedding as SB16 planes (logits of the mma variant) */
+    const void* emb_sb;                                              /* token embedding as SB16 planes (logits) */
     int64_t emb_plane;
-    int64_t use_mma;                                                 /* wts_decode_step_kernels: tensor-core matrix-vector phases */
     WtsDecodeCfg cfg;
-    int32_t n_layer, D, H, n_ctx, n_audio_ctx, n_slots, cap, lp_ld, qk_rows, n_steps, max_rows, prof_cap;
+    int32_t n_layer, D, H, n_ctx, n_audio_ctx, n_slots, cap, lp_ld, qk_rows, max_rows;
 } WtsDecodeSteps;
 
-/* Runs up to n_steps steps (stops early when every sequence is done).  After the launch sync[1] != 0 means the grid
- * barrier timed out (results invalid), sync[2] = steps completed.  Returns < 0 for unsupported dimensions. */
-int wts_decode_steps(const WtsDecodeSteps* p, void* stream);
-
-/* The same step as a chain of per-phase kernels under programmatic dependent launch (2 + 8 n_layer + 1 launches; meant to
- * be captured in a CUDA graph and replayed once per token): a kernel boundary costs less than a software grid barrier
- * across all SMs, and each kernel pulls its weight rows into L2 while its producer drains.  h_layers: HOST
- * copy of the layer table p->layers points to.  p->max_rows (1..32) sizes the grids and picks the rows-per-pass variant. */
+/* One step as a chain of per-phase kernels under programmatic dependent launch (2 + 8 n_layer + 1 launches; meant to
+ * be captured in a CUDA graph and replayed once per token): each kernel pulls its weight rows into L2 while its
+ * producer drains.  h_layers: HOST copy of the layer table p->layers points to.  p->max_rows (1..32) sizes the grids.
+ * Returns < 0 with a message for unsupported dimensions, or when the device has fewer than D / 16 SMs. */
 int wts_decode_step_kernels(const WtsDecodeSteps* p, const WtsDecLayer* h_layers, void* stream);
 
 /* Per-step decoder inputs from the token buffers: tok[b] = last token, pos[b] = its position,

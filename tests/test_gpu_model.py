@@ -255,23 +255,18 @@ def test_encoder_matches_oracle(tiny, backend):
         assert err <= TOL, (k, err)
 
 
-@pytest.mark.parametrize("small_rows", [32, 0, 2, -32, 320])
+@pytest.mark.parametrize("small_rows", [32, 0, 2])
 @pytest.mark.parametrize("backend", BACKENDS)
 def test_decode_windows_matches_oracle(tiny, backend, small_rows):
     """Same windows through the CUDA engine and the oracle engine: identical tokens, log-probs, no-speech
     probability and alignment-head cross-attention rows within 1e-3.  small_rows: 32 = every step by the lean small-
     batch kernels (wts_decode_step_kernels), 0 = every step by the per-operator tensor-core graph, 2 = that graph until
-    only two windows are left, then the lean kernels (the paths share caches and token state), -32 = every step by the
-    persistent cooperative kernel (wts_decode_steps), 320 = lean kernels with FP32-FMA matrix-vector phases instead of
-    mma.sync."""
+    only two windows are left, then the lean kernels (the paths share caches and token state)."""
     from whisper_timestamped.synthetic_audio import synthetic_speech
     from whisper_timestamped.tokenizer import get_tokenizer
     from whisper_timestamped.windows import make_decode_setup
     gm, om, oe = tiny
-    eng = _engine(gm, backend, keep_full_logprobs=True, small_batch_rows=min(32, abs(small_rows)))
-    if small_rows < 0:
-        eng.small_batch_mode = "persistent"           # the cooperative-kernel variant of the small-batch step
-    eng.small_batch_mma = small_rows != 320           # 320: the FP32-FMA variant of the lean kernels (default: mma.sync)
+    eng = _engine(gm, backend, keep_full_logprobs=True, small_batch_rows=small_rows)
     tok = get_tokenizer(True, num_languages=gm.num_languages, language="en", task="transcribe")
     setup = make_decode_setup(tok, gm.dims.n_text_ctx)
     audio = synthetic_speech(65.0, seed=33)
@@ -304,7 +299,7 @@ def test_decode_windows_matches_oracle(tiny, backend, small_rows):
                 want = float(oref[a.n_rows - 1, t])
                 got = a.last_row_logprobs(t)
                 assert (np.isinf(want) and np.isinf(got)) or abs(got - want) <= TOL
-    if abs(small_rows) in (32, 320):
+    if small_rows == 32:
         assert eng.small_batch_steps > 0
     elif small_rows == 0:
         assert eng.small_batch_steps == 0

@@ -1,7 +1,7 @@
 """Decode-step probe: milliseconds per decode step of a model at a fixed number of active windows, for the two step
 implementations that share the session state:
-  graph  : the per-operator step (tensor-core skinny GEMMs, one kernel per operator) replayed as ONE CUDA graph
-  steps  : the persistent small-batch kernel (wts_decode_steps, <= 32 active windows), `--steps` tokens per launch
+  graph    : the per-operator step (tensor-core skinny GEMMs, one kernel per operator) replayed as ONE CUDA graph
+  lean_mma : the lean small-batch step (wts_decode_step_kernels, <= 32 active windows) replayed as ONE CUDA graph
 
   python tools/step_probe.py --active 128,32,16,8,4,1 --cap 128 --steps 24
   ncu ... python tools/step_probe.py --eager --steps 2        (plain launches, for an ncu launch list)
@@ -25,7 +25,7 @@ def main():
     ap.add_argument("--active", type=str, default="128,32,16,8,4,1")
     ap.add_argument("--steps", type=int, default=24)
     ap.add_argument("--eager", action="store_true")
-    ap.add_argument("--only", default="graph,lean_mma,lean,steps")
+    ap.add_argument("--only", default="graph,lean_mma")
     args = ap.parse_args()
     import whisper_timestamped as wt
     from whisper_timestamped.engine import CudaEngine
@@ -81,47 +81,17 @@ def main():
             e1.record()
             torch.cuda.synchronize()
             res["graph_ms_per_step"] = round(e0.elapsed_time(e1) / args.steps, 3)
-        for name, mma in (("lean_mma", True), ("lean", False)):
-            if name in args.only.split(",") and ses["steps"] is not None and n_active <= eng.small_batch_rows:
-                reset(n_active)
-                eng.small_batch_mma = mma
-                graph = eng._lean_graph(ses, n_active)
-                for _ in range(3):
-                    graph.replay()
-                e0.record()
-                for _ in range(args.steps):
-                    graph.replay()
-                e1.record()
-                torch.cuda.synchronize()
-                res[name + "_ms_per_step"] = round(e0.elapsed_time(e1) / args.steps, 3)
-        if "steps" in args.only and ses["steps"] is not None and n_active <= eng.small_batch_rows:
+        if "lean_mma" in args.only.split(",") and ses["steps"] is not None and n_active <= eng.small_batch_rows:
             reset(n_active)
-            eng._run_steps(ses, 3, n_active)
-            torch.cuda.synchronize()
+            graph = eng._lean_graph(ses, n_active)
+            for _ in range(3):
+                graph.replay()
             e0.record()
-            eng._run_steps(ses, args.steps, n_active)
+            for _ in range(args.steps):
+                graph.replay()
             e1.record()
             torch.cuda.synchronize()
-            flags = ses["steps"]["keep"]["sync"].cpu().numpy()
-            res["steps_ms_per_step"] = round(e0.elapsed_time(e1) / max(1, int(flags[2])), 3)
-            res["steps_completed"] = int(flags[2])
-            res["barrier_timeout"] = int(flags[1])
-            # phase timeline of ONE step (CTA 0's %globaltimer after every grid barrier)
-            L = m.dims.n_text_layer
-            nb = 8 * L + 3
-            prof = torch.zeros(nb + 2, dtype=torch.int64, device="cuda")
-            p = ses["steps"]["args"]
-            p.prof, p.prof_cap = prof.data_ptr(), nb + 2
-            reset(n_active)
-            eng._run_steps(ses, 1, n_active)
-            torch.cuda.synchronize()
-            p.prof, p.prof_cap = None, 0
-            t = prof.cpu().numpy().astype(np.float64)
-            d = np.diff(t[: nb + 1]) / 1e3                      # microseconds per phase (incl. its closing barrier)
-            names = ["qkv", "self_attn", "out", "cross_q", "cross_attn", "cross_out", "fc1", "fc2"]
-            per = {n: round(float(d[1 + i: 1 + 8 * L: 8].mean()), 2) for i, n in enumerate(names)}
-            res["phase_us"] = dict(embed=round(float(d[0]), 2), **per, logits=round(float(d[1 + 8 * L]), 2),
-                                   select=round(float(d[2 + 8 * L]), 2), total=round(float(d.sum()), 1))
+            res["lean_mma_ms_per_step"] = round(e0.elapsed_time(e1) / args.steps, 3)
         out[n_active] = res
         print(f"active {n_active:4d} / cap {cap}: {res}", flush=True)
     print(json.dumps({"model": args.model, "cap": cap, "steps": args.steps, "ms": out}))

@@ -1,4 +1,4 @@
-// Device code shared by the per-kernel decode step (ops.cu) and the persistent decode-step kernel
+// Device code shared by the per-kernel decode step (ops.cu) and the lean small-batch decode step
 // (decode_steps.cu): block reductions, the one-pass fp16 cross-attention stream, and the fused
 // logit-filter / log-softmax / greedy-argmax of one sequence.
 #pragma once
@@ -153,8 +153,7 @@ __device__ __forceinline__ float ca_row_head(const float (&qf)[8], const __half*
 // Logit filters + log-softmax + greedy choice of ONE sequence by the whole CTA (any block size that is a multiple of
 // 32, <= 1024) — replaces SuppressBlank / SuppressTokens / ApplyTimestampRules / GreedyDecoder.update (upstream
 // whisper.decoding; rebuilt by the reference at T.py:1371-1393 and re-applied in hook_output_logits, T.py:871-875).
-// CG: read the logits / token state through ld.global.cg (the persistent kernel: they were written by other SMs
-// during this launch).  `last_full`: when this step reaches the decoding limit the whole filtered log-softmax row is
+// `last_full`: when this step reaches the decoding limit the whole filtered log-softmax row is
 // kept (one row per sequence) — the reference reads chunk_logprobs[-1][fallback_token] there (T.py:529-538, 735).
 struct SelectScratch {
     float red[32];
@@ -163,10 +162,6 @@ struct SelectScratch {
     int besti[32];
 };
 
-template <bool CG> __device__ __forceinline__ float ld_f(const float* p) { return CG ? __ldcg(p) : *p; }
-template <bool CG> __device__ __forceinline__ int ld_i(const int32_t* p) { return CG ? __ldcg(p) : *p; }
-
-template <bool CG>
 __device__ __forceinline__ void select_row(const float* x, const WtsDecodeCfg& cfg, const uint8_t* __restrict__ suppress,
                                            const uint8_t* __restrict__ blank, int32_t* tk, int32_t* n_tokens_b, int np,
                                            int32_t* done_b, float* logprobs_b, float* full_b, float* last_full_b,
@@ -175,18 +170,18 @@ __device__ __forceinline__ void select_row(const float* x, const WtsDecodeCfg& c
     // rows_only: only write the filtered log-softmax row to full_b[0 .. V) — no choice, no state update (what beam
     // search / sampling consume: upstream BeamSearchDecoder.update / GreedyDecoder.update work on these rows)
     const int T = blockDim.x;
-    const int nt = ld_i<CG>(n_tokens_b);
+    const int nt = *n_tokens_b;
     const int n = nt - np;                                   // sampled so far
     const int V = cfg.n_vocab, tsb = cfg.timestamp_begin, eot = cfg.eot;
     // ---- token history: position of the last sampled timestamp (parallel scan, no dependent chain)
     int last_pos = -1;
     for (int i = np + threadIdx.x; i < nt; i += T)
-        if (ld_i<CG>(tk + i) >= tsb) last_pos = i;           // ascending i per thread
+        if (tk[i] >= tsb) last_pos = i;                      // ascending i per thread
     last_pos = (int)block_reduce_max((float)last_pos, S.red);   // positions < 2^24: exact in float
     if (threadIdx.x == 0) {
-        const bool last_ts = n >= 1 && ld_i<CG>(tk + nt - 1) >= tsb;
-        const bool pen_ts = n < 2 || ld_i<CG>(tk + nt - 2) >= tsb;
-        const int tl = last_pos >= 0 ? ld_i<CG>(tk + last_pos) : -1;
+        const bool last_ts = n >= 1 && tk[nt - 1] >= tsb;
+        const bool pen_ts = n < 2 || tk[nt - 2] >= tsb;
+        const int tl = last_pos >= 0 ? tk[last_pos] : -1;
         int ts_limit = tsb;                                  // timestamps in [tsb, ts_limit) are forbidden
         if (tl >= 0) ts_limit = (last_ts && !pen_ts) ? tl : tl + 1;
         S.flags[0] = (n == 0);
@@ -218,7 +213,7 @@ __device__ __forceinline__ void select_row(const float* x, const WtsDecodeCfg& c
         for (int u = 0; u < UN; ++u) {
             const int v = v0 + u * T;
             const bool in = v < V;
-            xv[u] = in ? ld_f<CG>(x + v) : 0.f;
+            xv[u] = in ? x[v] : 0.f;
             const unsigned b = in ? (unsigned)__ldg(suppress + v) | (first ? (unsigned)__ldg(blank + v) : 0u) : 1u;
             bad |= (b != 0u ? 1u : 0u) << u;
         }
@@ -276,7 +271,7 @@ __device__ __forceinline__ void select_row(const float* x, const WtsDecodeCfg& c
     if (f1 != nullptr || f2 != nullptr) {
         for (int v = threadIdx.x; v < V; v += T) {
             const bool ok = !__ldg(suppress + v) && !(first && __ldg(blank + v)) && range_ok(v) && !(only_ts && v < tsb);
-            const float lp = ok ? ld_f<CG>(x + v) - lse : -CUDART_INF_F;
+            const float lp = ok ? x[v] - lse : -CUDART_INF_F;
             if (f1) f1[v] = lp;
             if (f2) f2[v] = lp;
         }

@@ -1,348 +1,36 @@
-// Persistent decode-step kernel for SMALL active batches (<= 32 windows still decoding).
+// Decoder step for SMALL active batches (<= 32 windows still decoding) as a chain of lean per-phase kernels.
 //
-// Why: a decoder step of large-v3 is ~355 dependent kernels when every operator is its own launch; at <= 32 active
-// windows each of them sits at its launch + prologue floor, far above the time the step's weight stream needs
-// from HBM.  Here ONE cooperative kernel (one CTA per SM, all co-resident) walks
+// Why: a decoder step of large-v3 is ~355 dependent kernels when every operator is its own launch; at a few active
+// windows each of them sits at its launch + prologue floor, far above the time the step's weight stream needs from HBM.
+// Here one step is 2 + 8 n_layer + 1 kernels,
 //     embed -> L x [LN+QKV | self-attn | out-proj | LN+Q | cross-attn | out-proj | LN+FC1+GELU | FC2] -> LN+logits -> select
-// for up to `n_steps` tokens, phases separated by a grid-wide barrier (one atomic + one polling thread per CTA).
+// launched with programmatic dependent launch and replayed as one CUDA graph: a kernel boundary under PDL is cheap,
+// and each matrix-vector kernel pulls its first weight rows into L2 while the previous kernel drains.  Cross-attention
+// K/V are streamed by the cross-attention kernel itself; nothing prefetches them.
 // Replaces, for the whole batch at once, upstream's DecodingTask._main_loop step + the reference's per-token hooks
 // (T.py:783-793 hook_attention_weights, 849-881 hook_output_logits).
 //
-// At <= 32 rows the GEMMs are weight-streaming matrix-vector products, so they run on the FP32 pipe (no tensor cores:
-// a 128-row tensor-core tile would be >= 75 % padding, and its tensor-map/barrier prologue costs a kernel that
-// short more than its math): a warp owns 4 output features, streams their float32 weight rows once (coalesced 512-byte loads, L1
-// bypassed), multiplies them with up to 16 activation rows staged in shared memory (LayerNorm fused into the
-// staging), and reduces over the lanes with a transposing butterfly that leaves every lane with its own outputs.
-// Weights of the NEXT phase are prefetched into L2 before each barrier, so HBM keeps streaming while CTAs wait.
-// Results are float32 throughout (weights float32 = the exact values the SB16 tensor-core path carries as hi + lo).
+// The matrix-vector phases run on mma.sync tensor cores with the SB16 weight planes (see lean_mma_kernel); attention,
+// LayerNorm statistics, the filters and the choice stay in float32.  The kernels find the active rows from the done
+// flags on the device, so one graph serves every step; only the grid sizes depend on the host's bound `max_rows`.
 #include "decode_common.cuh"
 
 namespace wts {
 
 constexpr int MG_THREADS = 256;
 constexpr int MG_WARPS = MG_THREADS / 32;
-constexpr int MG_MAXROWS = 32;          // active rows the staging buffer holds
-constexpr int MG_G = 4;                 // output features per warp task
+constexpr int MG_MAXROWS = 32;          // active rows a step handles
 constexpr int MG_MAXNI = 10;            // D / 128 <= 10 (D <= 1280)
 
 struct MgShared {
     int list[MG_MAXROWS];               // active slots, ascending
     int n_active;
-    int abort_flag;
-    int prof_idx;                       // next slot of the optional phase timeline (block 0 only)
-    unsigned long long* prof;
-    int prof_cap;
-    SelectScratch sel;
 };
 
-__device__ __forceinline__ float4 ldg_stream4(const float* p)
-{
-    float4 v;
-    asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];"
-                 : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
-    return v;
-}
 __device__ __forceinline__ float4 ldcg4(const float* p) { return __ldcg(reinterpret_cast<const float4*>(p)); }
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
-// ---- grid-wide barrier.  Arrivals are one release-add per CTA on a counter; the LAST arriver publishes the new
-// generation on a different 128-byte line, which is the only thing the other CTAs poll (acquire loads with a short
-// back-off) — polls never contend with the arriving atomics (polling the counter itself, or a flag array where every
-// CTA publishes its generation and warp 0 polls all of them, both keep the arrivals waiting on the polls).  sync[0] = arrivals, sync[1] = error flag, sync[2] = steps completed, sync[32] = generation.
-// A spin limit turns a would-be hang (a bug, or a grid that is not co-resident) into an error flag the host reports.
-__device__ __forceinline__ void grid_sync(uint32_t* sync, uint32_t& gen, MgShared& sh)
-{
-    __syncthreads();
-    gen += 1;
-    if (threadIdx.x == 0 && !sh.abort_flag) {
-        __threadfence();
-        uint32_t old;
-        asm volatile("atom.add.release.gpu.global.u32 %0, [%1], 1;" : "=r"(old) : "l"(sync) : "memory");
-        if (old + 1 == gen * gridDim.x) {
-            asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(sync + 32), "r"(gen) : "memory");
-        } else {
-            uint32_t g;
-            int spins = 0;
-            while (true) {
-                asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(g) : "l"(sync + 32) : "memory");
-                if (g >= gen) break;
-                __nanosleep(20);
-                if ((++spins & 1023) == 0) {
-                    uint32_t e;
-                    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(e) : "l"(sync + 1) : "memory");
-                    if (e != 0 || spins > (1 << 22)) {       // ~1 s of polling: a bug, or a grid that is not co-resident
-                        atomicExch(sync + 1, 1u);
-                        sh.abort_flag = 1;
-                        break;
-                    }
-                }
-            }
-        }
-        __threadfence();
-    }
-    if (threadIdx.x == 0 && sh.prof != nullptr && sh.prof_idx < sh.prof_cap) {   // phase timeline (probe runs only)
-        unsigned long long t;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-        sh.prof[sh.prof_idx++] = t;
-    }
-    __syncthreads();
-}
-
-// ---- transposing warp reduction: v[i] (i < NV) summed over the 32 lanes; afterwards lane l holds in v[0 .. NV/32)
-// the totals of logical indices l * (NV / 32) + j  (NV >= 32), or for NV = 16 in v[0] the total of index l >> 1.
-template <int N, int MASK>
-__device__ __forceinline__ void treduce_step(float* v, int lane)
-{
-    if constexpr (N > 1 && MASK >= 1) {
-        const bool up = (lane & MASK) != 0;
-#pragma unroll
-        for (int i = 0; i < N / 2; ++i) {
-            const float keep = up ? v[i + N / 2] : v[i];
-            const float send = up ? v[i] : v[i + N / 2];
-            v[i] = keep + __shfl_xor_sync(FULL_MASK, send, MASK);
-        }
-        treduce_step<N / 2, MASK / 2>(v, lane);
-    } else if constexpr (MASK >= 1) {
-        v[0] += __shfl_xor_sync(FULL_MASK, v[0], MASK);
-        treduce_step<1, MASK / 2>(v, lane);
-    }
-}
-
-// ---- staging of activation rows into shared memory (optionally LayerNorm'ed).  Warp w takes rows w, w + 8, ... of the
-// pass: all of its 16-byte cp.async.cg copies are issued back to back (one memory round trip for the whole staging;
-// .cg = through L2, the rows were produced by other SMs earlier in this launch), then it normalises its own rows in
-// place.  xs row r (pitch `ncols`) <- src[list[row_first + r], col0 .. col0 + ncols).  Ends with a CTA barrier.
-constexpr int MG_STAGE_FLOATS = MG_MAXROWS * 128 * MG_MAXNI;     // staging capacity: 32 rows x 1280 columns
-
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src)
-{
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
-}
-
-template <bool LN>
-__device__ __forceinline__ void stage_rows(const float* src, int64_t ld, int col0, int ncols, int row_first, int nrows,
-                                           const float* __restrict__ gam, const float* __restrict__ bet, const MgShared& sh,
-                                           float* xs)
-{
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int c4n = ncols >> 2;
-    const uint32_t xs_a = (uint32_t)__cvta_generic_to_shared(xs);
-    for (int r = warp; r < nrows; r += MG_WARPS) {
-        const float* g = src + (int64_t)sh.list[row_first + r] * ld + col0;
-        const uint32_t d = xs_a + (uint32_t)(r * ncols) * 4u;
-        for (int c4 = lane; c4 < c4n; c4 += 32) cp_async16(d + 16u * c4, g + 4 * c4);
-    }
-    asm volatile("cp.async.commit_group;" ::: "memory");
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
-    __syncwarp();
-    if (LN) {                                                // ncols == D: the whole row is here
-        const int NI = ncols >> 7;
-        for (int r = warp; r < nrows; r += MG_WARPS) {
-            float4* row = reinterpret_cast<float4*>(xs + (int64_t)r * ncols);
-            float4 v[MG_MAXNI];
-            float s = 0.f;
-#pragma unroll
-            for (int k = 0; k < MG_MAXNI; ++k)
-                if (k < NI) { v[k] = row[lane + 32 * k]; s += (v[k].x + v[k].y) + (v[k].z + v[k].w); }
-            const float mean = warp_sum(s) / (float)ncols;
-            float q = 0.f;
-#pragma unroll
-            for (int k = 0; k < MG_MAXNI; ++k)
-                if (k < NI) {
-                    const float a = v[k].x - mean, b = v[k].y - mean, c = v[k].z - mean, d = v[k].w - mean;
-                    q += (a * a + b * b) + (c * c + d * d);
-                }
-            const float rstd = 1.0f / sqrtf(warp_sum(q) / (float)ncols + 1e-5f);
-#pragma unroll
-            for (int k = 0; k < MG_MAXNI; ++k)
-                if (k < NI) {
-                    const float4 g = __ldg(reinterpret_cast<const float4*>(gam) + lane + 32 * k);
-                    const float4 b = __ldg(reinterpret_cast<const float4*>(bet) + lane + 32 * k);
-                    v[k].x = (v[k].x - mean) * rstd * g.x + b.x;
-                    v[k].y = (v[k].y - mean) * rstd * g.y + b.y;
-                    v[k].z = (v[k].z - mean) * rstd * g.z + b.z;
-                    v[k].w = (v[k].w - mean) * rstd * g.w + b.w;
-                    row[lane + 32 * k] = v[k];
-                }
-        }
-    }
-    __syncthreads();
-}
-
-// ---- one K chunk (NI * 128 columns) of a warp task: acc[g][b] += W[n0 + g, kc0 ...] . xs[b, ...]
-// The weight slices (4 features x one float4 per lane) run through a 4-slot register ring: three slices are always in
-// flight while the fourth is multiplied with the staged rows (RB shared-memory float4 loads, 16 FMAs each).
-template <int RB>
-__device__ __forceinline__ void gemv_slice(const float4 (&w)[MG_G], const float* xp, int pitch, float (&acc)[MG_G * RB])
-{
-    constexpr int HB = RB > 8 ? 4 : RB;                      // rows per batch of shared-memory loads (bounds live registers)
-#pragma unroll
-    for (int b0 = 0; b0 < RB; b0 += HB) {
-        float4 xv[HB];
-#pragma unroll
-        for (int b = 0; b < HB; ++b) xv[b] = *reinterpret_cast<const float4*>(xp + (b0 + b) * pitch);
-#pragma unroll
-        for (int b = 0; b < HB; ++b) {
-#pragma unroll
-            for (int g = 0; g < MG_G; ++g) {
-                float a = acc[g * RB + b0 + b];
-                a = fmaf(w[g].x, xv[b].x, a);
-                a = fmaf(w[g].y, xv[b].y, a);
-                a = fmaf(w[g].z, xv[b].z, a);
-                a = fmaf(w[g].w, xv[b].w, a);
-                acc[g * RB + b0 + b] = a;
-            }
-        }
-        asm volatile("" ::: "memory");                       // keep the next batch of loads behind this batch's FMAs
-    }
-}
-
-template <int RB>
-__device__ __forceinline__ void gemv_chunk(const float* __restrict__ W, int64_t ldw, int n0, int N, int kc0, int NI,
-                                           const float* xs, int pitch, float (&acc)[MG_G * RB])
-{
-    const int lane = threadIdx.x & 31;
-    const float* wp[MG_G];
-#pragma unroll
-    for (int g = 0; g < MG_G; ++g) wp[g] = W + (int64_t)min(n0 + g, N - 1) * ldw + kc0 + 4 * lane;
-    float4 w[4][MG_G];
-#pragma unroll
-    for (int u = 0; u < 3; ++u)
-        if (u < NI) {
-#pragma unroll
-            for (int g = 0; g < MG_G; ++g) w[u][g] = ldg_stream4(wp[g] + 128 * u);
-        }
-#pragma unroll 1
-    for (int i0 = 0; i0 < NI; i0 += 4) {
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-            const int i = i0 + u;
-            if (i + 3 < NI) {
-#pragma unroll
-                for (int g = 0; g < MG_G; ++g) w[(u + 3) & 3][g] = ldg_stream4(wp[g] + 128 * (i + 3));
-            }
-            if (i < NI) gemv_slice<RB>(w[u], xs + 4 * (lane + 32 * i), pitch, acc);
-        }
-    }
-}
-
 enum { EPI_STORE = 0, EPI_ADD = 1, EPI_GELU = 2 };
-
-// ---- epilogue of a warp task after the transposing reduction
-template <int RB>
-__device__ __forceinline__ void gemv_epilogue(float (&acc)[MG_G * RB], int n0, int N, int row0, const MgShared& sh,
-                                              const float* __restrict__ bias, float* out, int64_t ldo, int epi)
-{
-    const int lane = threadIdx.x & 31;
-    constexpr int NV = MG_G * RB;
-    treduce_step<NV, 16>(acc, lane);
-    constexpr int PER = NV >= 32 ? NV / 32 : 1;
-    const int base = NV >= 32 ? lane * PER : lane / (32 / (NV < 32 ? NV : 32));
-    const bool writer = NV >= 32 ? true : (lane % (32 / (NV < 32 ? NV : 32))) == 0;
-    if (!writer) return;
-#pragma unroll
-    for (int j = 0; j < PER; ++j) {
-        const int idx = base + j;
-        const int g = idx / RB, b = idx % RB;
-        const int n = n0 + g;
-        const int ri = row0 + b;
-        if (n < N && ri < sh.n_active) {
-            float t = acc[j] + (bias != nullptr ? __ldg(bias + n) : 0.f);
-            float* dst = out + (int64_t)sh.list[ri] * ldo + n;
-            if (epi == EPI_GELU) t = gelu_erf(t);
-            else if (epi == EPI_ADD) t += __ldcg(dst);
-            *dst = t;
-        }
-    }
-}
-
-// ---- a whole matrix-vector phase: out[row, n] = epi(sum_k W[n, k] * act[row, k] + bias[n]) for the active rows.
-// act rows come from `src` (global, K columns) staged chunk by chunk (D columns each) into shared memory, with
-// LayerNorm(gam, bet) fused when LN (then K == D).  Tasks (4 features) are dealt round-robin to the warps of the grid.
-template <int RB, bool LN>
-__device__ __noinline__ void gemv_phase(const float* __restrict__ W, int N, int K, int D, const float* __restrict__ bias,
-                                           const float* src, int64_t lds, const float* gam, const float* bet, float* out,
-                                           int64_t ldo, int epi, const MgShared& sh, float* xs)
-{
-    const int warp = threadIdx.x >> 5;
-    const int total_warps = gridDim.x * MG_WARPS;
-    const int gw = warp * gridDim.x + blockIdx.x;            // consecutive tasks land on different SMs
-    const int nA = sh.n_active;
-    const int ntasks = (N + MG_G - 1) / MG_G;
-    const int rounds = (ntasks + total_warps - 1) / total_warps;
-    const int npass = (nA + RB - 1) / RB;
-    // Either every pass's RB rows with all K columns fit the staging buffer (always when K == D): staged ONCE for all
-    // rounds and passes.  Or (FC2 with more than 8 active rows) each pass stages its own rows in chunks of Kc columns.
-    const bool once = npass * RB * K <= MG_STAGE_FLOATS;     // a pass reads RB rows of the buffer whatever nA is
-    const int Kc = once ? K : (MG_STAGE_FLOATS / (RB * D)) * D;
-    const int nchunks = (K + Kc - 1) / Kc;
-    if (once) stage_rows<LN>(src, lds, 0, K, 0, nA, gam, bet, sh, xs);
-    for (int rd = 0; rd < rounds; ++rd) {
-        const int t = gw + rd * total_warps;
-        const bool has = t < ntasks;
-        for (int ps = 0; ps < npass; ++ps) {
-            float acc[MG_G * RB];
-#pragma unroll
-            for (int i = 0; i < MG_G * RB; ++i) acc[i] = 0.f;
-            for (int c = 0; c < nchunks; ++c) {
-                const int kc = min(Kc, K - c * Kc);
-                if (!once) {
-                    __syncthreads();                         // previous chunk fully consumed
-                    stage_rows<false>(src, lds, c * Kc, kc, ps * RB, min(RB, nA - ps * RB), nullptr, nullptr, sh, xs);
-                }
-                if (has) gemv_chunk<RB>(W, K, t * MG_G, N, c * Kc, kc >> 7, once ? xs + (int64_t)ps * RB * K : xs, kc, acc);
-            }
-            if (has) gemv_epilogue<RB>(acc, t * MG_G, N, ps * RB, sh, bias, out, ldo, epi);
-        }
-    }
-}
-
-// L2 prefetch of the weight rows this warp will stream in a later phase
-__device__ __forceinline__ void prefetch_phase(const float* W, int N, int K, int max_rounds = 1 << 30)
-{
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int total_warps = gridDim.x * MG_WARPS;
-    const int gw = warp * gridDim.x + blockIdx.x;
-    const int ntasks = (N + MG_G - 1) / MG_G;
-    const int lines_per_row = K / 32;                        // 128-byte lines
-    for (int t = gw, r = 0; t < ntasks && r < max_rounds; t += total_warps, ++r) {
-        for (int ln = lane; ln < MG_G * lines_per_row; ln += 32) {
-            const int g = ln / lines_per_row, c = ln - g * lines_per_row;
-            const int n = min(t * MG_G + g, N - 1);
-            prefetch_l2(W + (int64_t)n * K + c * 32);
-        }
-    }
-}
-
-// At most this many active rows get their cross-attention K/V prefetched into L2 (a "few rows" step leaves HBM idle
-// during its matrix-vector phases).  The launcher lowers the cap further so that one layer's prefetched fp16 K + V fit
-// in half of the device's L2 (the other half keeps the weight rows the phases stream): large-v3 holds 7.7 MB per row,
-// so a 50 MB L2 takes 3 rows.
-constexpr int MG_KV_PREFETCH_ROWS = 8;
-
-__device__ __forceinline__ void prefetch_cross_kv(const WtsDecodeSteps& P, const WtsDecLayer& Lr, const MgShared& sh)
-{
-    const int64_t per_row = (int64_t)P.H * P.n_audio_ctx * 64 * 2;             // bytes of fp16 K (and of V) per row
-    const int64_t lines_row = per_row / 128;
-    const int64_t nthreads = (int64_t)gridDim.x * MG_THREADS, me = (int64_t)blockIdx.x * MG_THREADS + threadIdx.x;
-    for (int i = 0; i < sh.n_active; ++i) {
-        const char* k = reinterpret_cast<const char*>(Lr.cross_k16) + (int64_t)sh.list[i] * per_row;
-        const char* v = reinterpret_cast<const char*>(Lr.cross_v16) + (int64_t)sh.list[i] * per_row;
-        for (int64_t ln = me; ln < lines_row; ln += nthreads) {
-            prefetch_l2(k + ln * 128);
-            prefetch_l2(v + ln * 128);
-        }
-        // float32 K of the alignment heads of this layer
-        const int64_t al_row = (int64_t)P.n_slots * P.n_audio_ctx * 64 * 4;
-        const char* ka = reinterpret_cast<const char*>(Lr.cross_k_align) + (int64_t)sh.list[i] * al_row;
-        for (int h = 0; h < P.H; ++h) {
-            const int slot = __ldg(Lr.head_slot + h);
-            if (slot < 0) continue;
-            const int64_t lines = (int64_t)P.n_audio_ctx * 64 * 4 / 128;
-            for (int64_t ln = me; ln < lines; ln += nthreads) prefetch_l2(ka + (int64_t)slot * lines * 128 + ln * 128);
-        }
-    }
-}
 
 // ---- causal self-attention of ONE (row, head) by a warp; appends this position's K/V to the cache first.
 // `sc`: this warp's shared-memory scratch, n_ctx floats (scores, then probabilities).
@@ -437,140 +125,6 @@ __device__ __noinline__ void cross_attention_phase(const WtsDecodeSteps& P, cons
     }
 }
 
-template <int RB>
-__device__ void decode_layers_and_logits(const WtsDecodeSteps& P, MgShared& sh, float* xs, uint32_t& target, int kv_pf_rows)
-{
-    const int D = P.D, H = P.H;
-    const int warp = threadIdx.x >> 5;
-    const int total_warps = gridDim.x * MG_WARPS;
-    const int gw = warp * gridDim.x + blockIdx.x;
-    for (int li = 0; li < P.n_layer; ++li) {
-        const WtsDecLayer& Lr = P.layers[li];
-        // few active rows: pull this layer's cross-attention K/V into L2 now (the matrix-vector phases in between leave HBM
-        // idle), so the (row, head) streams of P5 — each a single CTA with limited bytes in flight — run at L2 latency
-        if (sh.n_active <= kv_pf_rows) prefetch_cross_kv(P, Lr, sh);
-        // P1: LN + QKV
-        gemv_phase<RB, true>(Lr.w_qkv, 3 * D, D, D, Lr.b_qkv, P.x, D, Lr.ln1_g, Lr.ln1_b, P.qkv, 3 * D, EPI_STORE, sh, xs);
-        prefetch_phase(Lr.w_o, D, D);
-        grid_sync(P.sync, target, sh);
-        // P2: self-attention, one warp per (row, head)
-        for (int t = gw; t < sh.n_active * H; t += total_warps) {
-            const int row = sh.list[t / H];
-            self_attention_task(P, Lr, row, t % H, __ldcg(P.n_tokens + row) - 1, xs + warp * P.n_ctx);
-        }
-        grid_sync(P.sync, target, sh);
-        // P3: out-projection + residual
-        gemv_phase<RB, false>(Lr.w_o, D, D, D, Lr.b_o, P.att, D, nullptr, nullptr, P.x, D, EPI_ADD, sh, xs);
-        prefetch_phase(Lr.w_cq, D, D);
-        grid_sync(P.sync, target, sh);
-        // P4: LN + cross query
-        gemv_phase<RB, true>(Lr.w_cq, D, D, D, Lr.b_cq, P.x, D, Lr.ln2_g, Lr.ln2_b, P.q, D, EPI_STORE, sh, xs);
-        prefetch_phase(Lr.w_co, D, D);
-        grid_sync(P.sync, target, sh);
-        // P5: cross-attention, one CTA per (row, head); scratch aliases the (idle) staging buffer
-        cross_attention_phase(P, Lr, sh, xs);
-        grid_sync(P.sync, target, sh);
-        // P6: cross out-projection + residual
-        gemv_phase<RB, false>(Lr.w_co, D, D, D, Lr.b_co, P.att, D, nullptr, nullptr, P.x, D, EPI_ADD, sh, xs);
-        prefetch_phase(Lr.w_fc1, 4 * D, D);
-        grid_sync(P.sync, target, sh);
-        // P7: LN + FC1 + GELU
-        gemv_phase<RB, true>(Lr.w_fc1, 4 * D, D, D, Lr.b_fc1, P.x, D, Lr.ln3_g, Lr.ln3_b, P.mid, 4 * D, EPI_GELU, sh, xs);
-        prefetch_phase(Lr.w_fc2, D, 4 * D);
-        grid_sync(P.sync, target, sh);
-        // P8: FC2 + residual (K = 4D in D-column chunks)
-        gemv_phase<RB, false>(Lr.w_fc2, D, 4 * D, D, Lr.b_fc2, P.mid, 4 * D, nullptr, nullptr, P.x, D, EPI_ADD, sh, xs);
-        if (li + 1 < P.n_layer) prefetch_phase(P.layers[li + 1].w_qkv, 3 * D, D);
-        grid_sync(P.sync, target, sh);
-    }
-    // final LN + tied-embedding logits
-    gemv_phase<RB, true>(P.emb, P.cfg.n_vocab, D, D, nullptr, P.x, D, P.ln_g, P.ln_b, P.logits, P.cfg.n_vocab, EPI_STORE, sh, xs);
-    grid_sync(P.sync, target, sh);
-}
-
-__device__ __noinline__ void select_phase(const WtsDecodeSteps& P, MgShared& sh)
-{
-    for (int i = blockIdx.x; i < sh.n_active; i += gridDim.x) {
-        const int row = sh.list[i];
-        select_row<true>(P.logits + (int64_t)row * P.cfg.n_vocab, P.cfg, P.suppress, P.blank,
-                         P.tokens + (int64_t)row * P.cfg.tokens_ld, P.n_tokens + row, __ldg(P.n_prompt + row), P.done + row,
-                         P.logprobs + (int64_t)row * P.lp_ld,
-                         P.full != nullptr ? P.full + (int64_t)row * P.lp_ld * P.cfg.n_vocab : nullptr,
-                         P.last_full != nullptr ? P.last_full + (int64_t)row * P.cfg.n_vocab : nullptr, sh.sel);
-        __syncthreads();
-    }
-}
-
-// RB = activation rows per weight pass (4, 8 or 16): chosen by the host from the number of active rows at launch
-// (it only shrinks during a launch); more rows than RB simply take several passes.
-template <int RB>
-__global__ void __launch_bounds__(MG_THREADS, 1)
-decode_steps_kernel(const WtsDecodeSteps P, const int kv_pf_rows)
-{
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    MgShared& sh = *reinterpret_cast<MgShared*>(smem_raw);
-    float* xs = reinterpret_cast<float*>(smem_raw + 1024);    // [MG_MAXROWS][D] staging (aliased by the attention scratch)
-    static_assert(sizeof(MgShared) <= 1024, "MgShared must fit its slot");
-    uint32_t target = 0;
-    if (threadIdx.x == 0) {
-        sh.abort_flag = 0;
-        sh.prof = blockIdx.x == 0 ? reinterpret_cast<unsigned long long*>(P.prof) : nullptr;
-        sh.prof_cap = P.prof_cap;
-        sh.prof_idx = 0;
-        if (sh.prof != nullptr && sh.prof_cap > 0) {
-            unsigned long long t;
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-            sh.prof[sh.prof_idx++] = t;
-        }
-    }
-    const int D = P.D;
-
-    for (int step = 0; step < P.n_steps; ++step) {
-        // ---- active rows (every CTA builds the same list; `done` was settled before the last barrier)
-        __syncthreads();
-        if (threadIdx.x < 32) {
-            int count = 0;
-            for (int b0 = 0; b0 < P.cap; b0 += 32) {
-                const int b = b0 + threadIdx.x;
-                const bool act = b < P.cap && __ldcg(P.done + b) == 0;
-                const unsigned bal = __ballot_sync(FULL_MASK, act);
-                const int at = count + __popc(bal & ((1u << threadIdx.x) - 1u));
-                if (act && at < MG_MAXROWS) sh.list[at] = b;
-                count += __popc(bal);
-            }
-            if (threadIdx.x == 0) sh.n_active = count;
-        }
-        __syncthreads();
-        const int nA = sh.n_active;
-        if (nA == 0 || nA > MG_MAXROWS || sh.abort_flag) break;         // uniform over the grid
-
-        // ---- embed: x[row] = token_embedding[last token] + positional_embedding[its position]
-        for (int i = blockIdx.x; i < nA; i += gridDim.x) {
-            const int row = sh.list[i];
-            const int nt = __ldcg(P.n_tokens + row);
-            const int tok = __ldcg(P.tokens + (int64_t)row * P.cfg.tokens_ld + nt - 1);
-            const float* e = P.emb + (int64_t)tok * D;
-            const float* p = P.pos + (int64_t)(nt - 1) * D;
-            for (int c = threadIdx.x; c < D; c += MG_THREADS) P.x[(int64_t)row * D + c] = __ldg(e + c) + __ldg(p + c);
-        }
-        if (step == 0) prefetch_phase(P.layers[0].w_qkv, 3 * D, D);
-        grid_sync(P.sync, target, sh);
-
-        decode_layers_and_logits<RB>(P, sh, xs, target, kv_pf_rows);
-
-        // ---- filters + log-softmax + greedy choice: one CTA per active row
-        select_phase(P, sh);
-        if (blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(P.sync + 2, 1u);   // steps completed
-        grid_sync(P.sync, target, sh);
-    }
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// The same step as a chain of LEAN kernels (one per phase), launched with programmatic dependent launch and replayed
-// as one CUDA graph.  A software grid barrier costs microseconds (atomics + polling through L2), and the persistent
-// kernel needs 259 of them per step even for one active window (tools/step_probe.py times both variants).  A kernel
-// boundary under PDL is cheaper, and the next kernel's independent prologue
-// (pulling its weight rows into L2) runs while the previous one drains.  Same device code per phase.
 __device__ __forceinline__ void build_row_list(const WtsDecodeSteps& P, MgShared& sh)
 {
     if (threadIdx.x < 32) {
@@ -583,7 +137,7 @@ __device__ __forceinline__ void build_row_list(const WtsDecodeSteps& P, MgShared
             if (act && at < MG_MAXROWS) sh.list[at] = b;
             count += __popc(bal);
         }
-        if (threadIdx.x == 0) { sh.n_active = count <= MG_MAXROWS ? count : 0; sh.abort_flag = 0; sh.prof = nullptr; }
+        if (threadIdx.x == 0) sh.n_active = count <= MG_MAXROWS ? count : 0;
     }
     __syncthreads();
 }
@@ -600,22 +154,6 @@ lean_embed_kernel(const WtsDecodeSteps P)
     const float* e = P.emb + (int64_t)tok * P.D;
     const float* p = P.pos + (int64_t)(nt - 1) * P.D;
     for (int c = threadIdx.x; c < P.D; c += MG_THREADS) P.x[(int64_t)row * P.D + c] = __ldg(e + c) + __ldg(p + c);
-}
-
-template <int RB, bool LN>
-__global__ void __launch_bounds__(MG_THREADS, 1)
-lean_gemv_kernel(const WtsDecodeSteps P, const float* __restrict__ W, int N, int K, const float* __restrict__ bias,
-                 const float* src, int64_t lds, const float* gam, const float* bet, float* out, int64_t ldo, int epi)
-{
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    MgShared& sh = *reinterpret_cast<MgShared*>(smem_raw);
-    float* xs = reinterpret_cast<float*>(smem_raw + 1024);
-    pdl_launch();
-    prefetch_phase(W, N, K, 3);                              // this CTA's first weight rows -> L2 while the producer drains
-    pdl_wait();
-    build_row_list(P, sh);
-    if (sh.n_active == 0) return;
-    gemv_phase<RB, LN>(W, N, K, P.D, bias, src, lds, gam, bet, out, ldo, epi, sh, xs);
 }
 
 __global__ void __launch_bounds__(MG_THREADS)
@@ -656,17 +194,16 @@ lean_select_kernel(const WtsDecodeSteps P)
     pdl_wait();
     const int row = blockIdx.x;
     if (row >= P.cap || P.done[row] != 0) return;
-    select_row<false>(P.logits + (int64_t)row * P.cfg.n_vocab, P.cfg, P.suppress, P.blank, P.tokens + (int64_t)row * P.cfg.tokens_ld,
-                      P.n_tokens + row, P.n_prompt[row], P.done + row, P.logprobs + (int64_t)row * P.lp_ld,
-                      P.full != nullptr ? P.full + (int64_t)row * P.lp_ld * P.cfg.n_vocab : nullptr,
-                      P.last_full != nullptr ? P.last_full + (int64_t)row * P.cfg.n_vocab : nullptr, S);
+    select_row(P.logits + (int64_t)row * P.cfg.n_vocab, P.cfg, P.suppress, P.blank, P.tokens + (int64_t)row * P.cfg.tokens_ld,
+               P.n_tokens + row, P.n_prompt[row], P.done + row, P.logprobs + (int64_t)row * P.lp_ld,
+               P.full != nullptr ? P.full + (int64_t)row * P.lp_ld * P.cfg.n_vocab : nullptr,
+               P.last_full != nullptr ? P.last_full + (int64_t)row * P.cfg.n_vocab : nullptr, S);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// Tensor-core variant of the lean matrix-vector phase: mma.sync.m16n8k16 (bf16 in, float32 accumulate) with the same
-// 3-term split-bf16 product as the wgmma GEMMs (hi*hi + lo*hi + hi*lo), but none of their per-kernel set-up (no
-// mbarrier ring, no tensor maps, no cluster): at 5..32 active windows the FP32-pipe version above is bound by shared-memory
-// loads (an LDS.128 per 16 FMAs), this one by the weight stream.
+// The lean matrix-vector phase: mma.sync.m16n8k16 (bf16 in, float32 accumulate) with the same 3-term split-bf16
+// product as the wgmma GEMMs (hi*hi + lo*hi + hi*lo), but none of their per-kernel set-up (no mbarrier ring, no tensor
+// maps, no cluster), so at a few active windows it is bound by the weight stream.
 //  * a CTA owns 8 output features per task; its 8 warps split K; each lane's weight fragment for TWO MMAs is ONE 16-byte
 //    load (8 consecutive k of feature n0 + lane/4, both SB16 planes) — made possible by a PERMUTED k order inside every
 //    32-k block: activations are staged as bf16x2 words with word 4 s + q <- k = 8 q + 2 s + {0, 1} (tests/dtw_kernel_model.py
@@ -900,7 +437,7 @@ lean_mma_kernel(const WtsDecodeSteps P, const __nv_bfloat16* __restrict__ Whi, i
 }
 
 template <int MT>
-static int launch_lean_step_mma(const WtsDecodeSteps& P, const WtsDecLayer* h_layers, int n_sm, cudaStream_t st)
+static int launch_lean_step(const WtsDecodeSteps& P, const WtsDecLayer* h_layers, int n_sm, cudaStream_t st)
 {
     const int D = P.D, H = P.H, V = P.cfg.n_vocab;
     const int pitchW = (D + 8) >> 1;
@@ -942,102 +479,13 @@ static int launch_lean_step_mma(const WtsDecodeSteps& P, const WtsDecLayer* h_la
     return 0;
 }
 
-template <int RB>
-static int launch_lean_step(const WtsDecodeSteps& P, const WtsDecLayer* h_layers, int n_sm, cudaStream_t st)
-{
-    const int D = P.D, H = P.H, V = P.cfg.n_vocab;
-    const size_t stage = (size_t)MG_STAGE_FLOATS * sizeof(float) + 1024;
-    const size_t sm_self = (size_t)MG_WARPS * P.n_ctx * sizeof(float) + 1024;
-    const size_t sm_cross = sizeof(CaScratch) + 1024;
-    static bool attr = false;
-    if (!attr) {
-        WTS_CUDA_CHECK(cudaFuncSetAttribute(lean_gemv_kernel<RB, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)stage));
-        WTS_CUDA_CHECK(cudaFuncSetAttribute(lean_gemv_kernel<RB, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)stage));
-        attr = true;
-    }
-    const dim3 g_gemv(n_sm), blk(MG_THREADS);
-    const dim3 g_self((P.max_rows * H + MG_WARPS - 1) / MG_WARPS), g_cross(P.max_rows * H);
-    WTS_CUDA_CHECK(launch_pdl(lean_embed_kernel, dim3(P.cap), blk, 0, st, P));
-    const float* nof = nullptr;
-    for (int li = 0; li < P.n_layer; ++li) {
-        const WtsDecLayer& L = h_layers[li];
-        const WtsDecLayer* dL = P.layers + li;
-        WTS_CUDA_CHECK(launch_pdl(lean_gemv_kernel<RB, true>, g_gemv, blk, stage, st, P, L.w_qkv, 3 * D, D, L.b_qkv, (const float*)P.x,
-                                  (int64_t)D, L.ln1_g, L.ln1_b, P.qkv, (int64_t)(3 * D), (int)EPI_STORE));
-        WTS_CUDA_CHECK(launch_pdl(lean_self_attn_kernel, g_self, blk, sm_self, st, P, dL));
-        WTS_CUDA_CHECK(launch_pdl(lean_gemv_kernel<RB, false>, g_gemv, blk, stage, st, P, L.w_o, D, D, L.b_o, (const float*)P.att,
-                                  (int64_t)D, nof, nof, P.x, (int64_t)D, (int)EPI_ADD));
-        WTS_CUDA_CHECK(launch_pdl(lean_gemv_kernel<RB, true>, g_gemv, blk, stage, st, P, L.w_cq, D, D, L.b_cq, (const float*)P.x,
-                                  (int64_t)D, L.ln2_g, L.ln2_b, P.q, (int64_t)D, (int)EPI_STORE));
-        WTS_CUDA_CHECK(launch_pdl(lean_cross_attn_kernel, g_cross, blk, sm_cross, st, P, dL));
-        WTS_CUDA_CHECK(launch_pdl(lean_gemv_kernel<RB, false>, g_gemv, blk, stage, st, P, L.w_co, D, D, L.b_co, (const float*)P.att,
-                                  (int64_t)D, nof, nof, P.x, (int64_t)D, (int)EPI_ADD));
-        WTS_CUDA_CHECK(launch_pdl(lean_gemv_kernel<RB, true>, g_gemv, blk, stage, st, P, L.w_fc1, 4 * D, D, L.b_fc1, (const float*)P.x,
-                                  (int64_t)D, L.ln3_g, L.ln3_b, P.mid, (int64_t)(4 * D), (int)EPI_GELU));
-        WTS_CUDA_CHECK(launch_pdl(lean_gemv_kernel<RB, false>, g_gemv, blk, stage, st, P, L.w_fc2, D, 4 * D, L.b_fc2, (const float*)P.mid,
-                                  (int64_t)(4 * D), nof, nof, P.x, (int64_t)D, (int)EPI_ADD));
-    }
-    WTS_CUDA_CHECK(launch_pdl(lean_gemv_kernel<RB, true>, g_gemv, blk, stage, st, P, P.emb, V, D, nof, (const float*)P.x, (int64_t)D,
-                              P.ln_g, P.ln_b, P.logits, (int64_t)V, (int)EPI_STORE));
-    WTS_CUDA_CHECK(launch_pdl(lean_select_kernel, dim3(P.cap), dim3(LEAN_SELECT_THREADS), 0, st, P));
-    return 0;
-}
-
 }  // namespace wts
 
 using namespace wts;
 
-extern "C" int wts_decode_steps(const WtsDecodeSteps* p, void* stream)
-{
-    if (!p) { set_error("wts_decode_steps: null argument"); return -2; }
-    const WtsDecodeSteps& P = *p;
-    if (P.D % 128 != 0 || P.D > 128 * MG_MAXNI || P.D != P.H * 64) {
-        set_error("wts_decode_steps: n_text_state %d not supported (multiple of 128, <= %d, 64 per head)", P.D, 128 * MG_MAXNI);
-        return -2;
-    }
-    if (P.max_rows > MG_MAXROWS) { set_error("wts_decode_steps: at most %d active rows", MG_MAXROWS); return -2; }
-    if (P.n_steps <= 0) return 0;
-    cudaStream_t st = (cudaStream_t)stream;
-    static int n_sm = 0, l2_bytes = 0;
-    static size_t smem_set = 0;
-    if (n_sm == 0) {
-        int dev = 0;
-        WTS_CUDA_CHECK(cudaGetDevice(&dev));
-        WTS_CUDA_CHECK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
-        WTS_CUDA_CHECK(cudaDeviceGetAttribute(&l2_bytes, cudaDevAttrL2CacheSize, dev));
-    }
-    const int64_t kv_row_bytes = 2 * (int64_t)P.H * P.n_audio_ctx * 64 * 2;     // fp16 K + V of one row, one layer
-    int kv_pf_rows = (int)((int64_t)l2_bytes / 2 / kv_row_bytes);
-    if (kv_pf_rows > MG_KV_PREFETCH_ROWS) kv_pf_rows = MG_KV_PREFETCH_ROWS;
-    const size_t stage = (size_t)MG_STAGE_FLOATS * sizeof(float);             // gemv_phase sizes its chunks for this capacity
-    size_t smem = stage > sizeof(CaScratch) ? stage : sizeof(CaScratch);
-    const size_t sa = (size_t)MG_WARPS * P.n_ctx * sizeof(float);             // self-attention score scratch
-    if (sa > smem) smem = sa;
-    smem += 1024;
-    if (smem > 227 * 1024) { set_error("wts_decode_steps: %zu bytes of shared memory needed", smem); return -2; }
-    if (smem > smem_set) {
-        WTS_CUDA_CHECK(cudaFuncSetAttribute(decode_steps_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        WTS_CUDA_CHECK(cudaFuncSetAttribute(decode_steps_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        WTS_CUDA_CHECK(cudaFuncSetAttribute(decode_steps_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        smem_set = smem;
-    }
-    WTS_CUDA_CHECK(cudaMemsetAsync(P.sync, 0, 64 * sizeof(uint32_t), st));
-    void* args[] = {const_cast<WtsDecodeSteps*>(p), &kv_pf_rows};
-    const void* fn = P.max_rows <= 4 ? (const void*)decode_steps_kernel<4>
-                   : P.max_rows <= 8 ? (const void*)decode_steps_kernel<8> : (const void*)decode_steps_kernel<16>;
-    WTS_CUDA_CHECK(cudaLaunchCooperativeKernel(fn, dim3(n_sm), dim3(MG_THREADS), args, smem, st));
-    return 0;
-}
-
-static bool D_ok_for_mma(const WtsDecodeSteps& P)
-{
-    // K chunks of D columns, 32-k blocks, at most two 8-feature tasks per CTA for the 4D-wide FC2, SB16 planes present
-    return P.D % 128 == 0 && P.emb_sb != nullptr && (P.D / MM_TASK_N) <= 2 * 132;
-}
-
-// One decoder step as a chain of per-phase kernels (same arithmetic as wts_decode_steps; see the comment above
-// lean_embed_kernel).  h_layers: HOST copy of the layer table (weight pointers become kernel arguments).  Capturable in a
-// CUDA graph: no host synchronisation, no memset.  2 + 8 n_layer + 1 launches.
+// One decoder step as a chain of per-phase kernels (see the comment at the top).  h_layers: HOST copy of the layer
+// table (weight pointers become kernel arguments).  Capturable in a CUDA graph: no host synchronisation, no memset.
+// 2 + 8 n_layer + 1 launches.
 extern "C" int wts_decode_step_kernels(const WtsDecodeSteps* p, const WtsDecLayer* h_layers, void* stream)
 {
     if (!p || !h_layers) { set_error("wts_decode_step_kernels: null argument"); return -2; }
@@ -1048,18 +496,19 @@ extern "C" int wts_decode_step_kernels(const WtsDecodeSteps* p, const WtsDecLaye
     }
     if (P.max_rows > MG_MAXROWS || P.max_rows < 1) { set_error("wts_decode_step_kernels: 1..%d active rows", MG_MAXROWS); return -2; }
     if ((size_t)MG_WARPS * P.n_ctx * sizeof(float) + 1024 > 48 * 1024) { set_error("wts_decode_step_kernels: n_text_ctx too large"); return -2; }
+    if (P.emb_sb == nullptr) { set_error("wts_decode_step_kernels: no SB16 token embedding"); return -2; }
     static int n_sm = 0;
     if (n_sm == 0) {
         int dev = 0;
         WTS_CUDA_CHECK(cudaGetDevice(&dev));
         WTS_CUDA_CHECK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
     }
-    cudaStream_t st = (cudaStream_t)stream;
-    if (P.use_mma) {
-        if (D_ok_for_mma(P)) return P.max_rows <= 16 ? launch_lean_step_mma<1>(P, h_layers, n_sm, st)
-                                                     : launch_lean_step_mma<2>(P, h_layers, n_sm, st);
+    // lean_mma_kernel's grid is one CTA per SM, and with K = 4 D (FC2) a CTA keeps at most two 8-feature tasks
+    // across the K chunks: fewer than D / 16 SMs would leave FC2 outputs uncomputed
+    if (P.D / MM_TASK_N > 2 * n_sm) {
+        set_error("wts_decode_step_kernels: n_text_state %d needs at least %d SMs, the device has %d", P.D, P.D / 16, n_sm);
+        return -2;
     }
-    if (P.max_rows <= 4) return launch_lean_step<4>(P, h_layers, n_sm, st);
-    if (P.max_rows <= 8) return launch_lean_step<8>(P, h_layers, n_sm, st);
-    return launch_lean_step<16>(P, h_layers, n_sm, st);
+    cudaStream_t st = (cudaStream_t)stream;
+    return P.max_rows <= 16 ? launch_lean_step<1>(P, h_layers, n_sm, st) : launch_lean_step<2>(P, h_layers, n_sm, st);
 }

@@ -385,10 +385,10 @@ decode_select_kernel(float* logits, int64_t ldl, const WtsDecodeCfg cfg,
     __shared__ SelectScratch S;
     const int b = blockIdx.x;
     if (done[b]) return;
-    select_row<false>(logits + (int64_t)b * ldl, cfg, suppress, blank, tokens + (int64_t)b * cfg.tokens_ld, n_tokens + b,
-                      n_prompt[b], done + b, logprobs + (int64_t)b * lp_ld,
-                      full != nullptr ? full + (int64_t)b * lp_ld * cfg.n_vocab : nullptr,
-                      last_full != nullptr ? last_full + (int64_t)b * cfg.n_vocab : nullptr, S);
+    select_row(logits + (int64_t)b * ldl, cfg, suppress, blank, tokens + (int64_t)b * cfg.tokens_ld, n_tokens + b,
+               n_prompt[b], done + b, logprobs + (int64_t)b * lp_ld,
+               full != nullptr ? full + (int64_t)b * lp_ld * cfg.n_vocab : nullptr,
+               last_full != nullptr ? last_full + (int64_t)b * cfg.n_vocab : nullptr, S);
 }
 
 // filtered log-softmax rows only (beam search / sampling): one CTA per sequence, no state update
@@ -398,8 +398,8 @@ filtered_logprobs_kernel(const float* logits, int64_t ldl, const WtsDecodeCfg cf
 {
     __shared__ SelectScratch S;
     const int b = blockIdx.x;
-    select_row<false>(logits + (int64_t)b * ldl, cfg, suppress, blank, tokens + (int64_t)b * cfg.tokens_ld, n_tokens + b,
-                      n_prompt[b], nullptr, nullptr, out + (int64_t)b * cfg.n_vocab, nullptr, S, true);
+    select_row(logits + (int64_t)b * ldl, cfg, suppress, blank, tokens + (int64_t)b * cfg.tokens_ld, n_tokens + b,
+               n_prompt[b], nullptr, nullptr, out + (int64_t)b * cfg.n_vocab, nullptr, S, true);
 }
 
 __global__ void step_inputs_kernel(const int32_t* tokens, int ld, const int32_t* n_tokens,

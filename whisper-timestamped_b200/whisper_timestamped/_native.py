@@ -63,9 +63,7 @@ class DecodeCfg(ctypes.Structure):
 class DecLayer(ctypes.Structure):
     """Mirror of `WtsDecLayer`."""
     _fields_ = [(n, ctypes.c_void_p) for n in (
-        "ln1_g", "ln1_b", "w_qkv", "b_qkv", "w_o", "b_o",
-        "ln2_g", "ln2_b", "w_cq", "b_cq", "w_co", "b_co",
-        "ln3_g", "ln3_b", "w_fc1", "b_fc1", "w_fc2", "b_fc2",
+        "ln1_g", "ln1_b", "b_qkv", "b_o", "ln2_g", "ln2_b", "b_cq", "b_co", "ln3_g", "ln3_b", "b_fc1", "b_fc2",
         "self_k", "self_v", "cross_k16", "cross_v16", "cross_k_align", "head_slot",
         "sb_qkv", "sb_o", "sb_cq", "sb_co", "sb_fc1", "sb_fc2")] + [(n, ctypes.c_int64) for n in (
         "pl_qkv", "pl_o", "pl_cq", "pl_co", "pl_fc1", "pl_fc2")]
@@ -76,10 +74,9 @@ class DecodeSteps(ctypes.Structure):
     _fields_ = [(n, ctypes.c_void_p) for n in (
         "layers", "emb", "pos", "ln_g", "ln_b", "tokens", "n_tokens", "n_prompt", "done",
         "logprobs", "full", "last_full", "qk_buf", "suppress", "blank",
-        "x", "qkv", "att", "q", "mid", "logits", "sync", "prof", "emb_sb")] + [("emb_plane", ctypes.c_int64),
-                                                                              ("use_mma", ctypes.c_int64), ("cfg", DecodeCfg)] + [(n, ctypes.c_int32) for n in (
-        "n_layer", "D", "H", "n_ctx", "n_audio_ctx", "n_slots", "cap", "lp_ld", "qk_rows", "n_steps", "max_rows",
-        "prof_cap")]
+        "x", "qkv", "att", "q", "mid", "logits", "emb_sb")] + [("emb_plane", ctypes.c_int64), ("cfg", DecodeCfg)] + [
+        (n, ctypes.c_int32) for n in ("n_layer", "D", "H", "n_ctx", "n_audio_ctx", "n_slots", "cap", "lp_ld", "qk_rows",
+                                      "max_rows")]
 
 
 def _load():
@@ -126,8 +123,6 @@ def _load():
     lib.wts_decode_select.argtypes = [vp, i64, ctypes.POINTER(DecodeCfg), vp, vp, vp, vp, vp, vp, vp, i32, vp, vp, i32, vp]
     lib.wts_filtered_logprobs.argtypes = [vp, i64, ctypes.POINTER(DecodeCfg), vp, vp, vp, vp, vp, vp, i32, vp]
     lib.wts_filtered_logprobs.restype = ctypes.c_int
-    lib.wts_decode_steps.argtypes = [ctypes.POINTER(DecodeSteps), vp]
-    lib.wts_decode_steps.restype = ctypes.c_int
     lib.wts_decode_step_kernels.argtypes = [ctypes.POINTER(DecodeSteps), vp, vp]
     lib.wts_decode_step_kernels.restype = ctypes.c_int
     lib.wts_step_inputs.argtypes = [vp, i32, vp, vp, vp, i32, vp, vp, vp, vp, vp]
@@ -147,7 +142,7 @@ EXPORTED_SYMBOLS = [
     "wts_version", "wts_last_error", "wts_dtw_dir_words", "wts_dtw_bnd_doubles",
     "wts_attn_prep_batch", "wts_dtw_batch", "wts_dtw_batch_sized", "wts_disfluency_starts", "wts_gemm", "wts_to_sb16", "wts_layernorm", "wts_softmax_rows",
     "wts_frames", "wts_power", "wts_logmel_max", "wts_logmel_finish", "wts_window_gather", "wts_embed",
-    "wts_gather_rows", "wts_decoder_attention", "wts_kv_append", "wts_decode_select", "wts_filtered_logprobs", "wts_decode_steps", "wts_decode_step_kernels", "wts_step_inputs",
+    "wts_gather_rows", "wts_decoder_attention", "wts_kv_append", "wts_decode_select", "wts_filtered_logprobs", "wts_decode_step_kernels", "wts_step_inputs",
     "wts_softmax_pick", "wts_logprob_gather", "wts_cross_kv_pack", "wts_cross_attention_f16", "wts_enc_attention",
 ]
 

@@ -55,11 +55,7 @@ class CudaEngine:
         self.small_batch_rows = min(32, int(os.environ.get("WTS_SMALL_BATCH_ROWS", "8")) if small_batch_rows is None
                                     else int(small_batch_rows))
         self.small_batch_steps = 0
-        # how the small-batch steps run: "lean" = chain of per-phase kernels replayed as a CUDA graph (default),
-        # "persistent" = one cooperative kernel with software grid barriers (slower: a software grid barrier costs microseconds)
-        self.small_batch_mode = os.environ.get("WTS_SMALL_BATCH_MODE", "lean")
-        # matrix-vector phases of the lean kernels on mma.sync tensor cores (split-bf16, 3 terms) instead of FP32 FMAs
-        self.small_batch_mma = os.environ.get("WTS_SMALL_BATCH_MMA", "1") != "0"
+        self.decode_steps_run = 0
         self._graphs = {}
         self.profile = False            # when set, phases are bracketed with CUDA events (stage_ms())
         self._events = []
@@ -297,18 +293,27 @@ class CudaEngine:
             self.launches += 2
 
     def _alloc_decoder_state(self, B, R):
+        """Decoder state of B sequences: the cross-attention K/V buffers, self-attention K/V caches and the activation
+        buffers of R query rows."""
         d, dev = self.dims, self.dev
         D, H, L = d.n_text_state, d.n_text_head, d.n_text_layer
         f32 = dict(dtype=torch.float32, device=dev)
+        st8 = self._alloc_cross_state(B)
+        st8.update(hs=SB16(R, D, dev), att=SB16(R, D, dev), mid=SB16(R, 4 * D, dev),
+                   qkv=torch.empty((R, 3 * D), **f32), q=torch.empty((R, D), **f32),
+                   sk=[torch.zeros((B, H, d.n_text_ctx, 64), **f32) for _ in range(L)],
+                   sv=[torch.zeros((B, H, d.n_text_ctx, 64), **f32) for _ in range(L)])
+        return st8
+
+    def _alloc_cross_state(self, B):
+        """Cross-attention K/V buffers for B windows (also the staging area of windows admitted into a session)."""
+        d, dev = self.dims, self.dev
+        H, L = d.n_text_head, d.n_text_layer
         return dict(
-            hs=SB16(R, D, dev), att=SB16(R, D, dev), mid=SB16(R, 4 * D, dev),
-            qkv=torch.empty((R, 3 * D), **f32), q=torch.empty((R, D), **f32),
-            sk=[torch.zeros((B, H, d.n_text_ctx, 64), **f32) for _ in range(L)],
-            sv=[torch.zeros((B, H, d.n_text_ctx, 64), **f32) for _ in range(L)],
             ck=[torch.empty((B, H, N_CTX_AUDIO, 64), dtype=torch.float16, device=dev) for _ in range(L)],
             cv=[torch.empty((B, H, N_CTX_AUDIO, 64), dtype=torch.float16, device=dev) for _ in range(L)],
-            ckal=[torch.empty((B, max(1, len(self.m.heads)), N_CTX_AUDIO, 64), **f32) for _ in range(L)],
-            kvtmp=torch.empty((B, H, N_CTX_AUDIO, 64), **f32))
+            ckal=[torch.empty((B, max(1, len(self.m.heads)), N_CTX_AUDIO, 64), dtype=torch.float32, device=dev) for _ in range(L)],
+            kvtmp=torch.empty((B, H, N_CTX_AUDIO, 64), dtype=torch.float32, device=dev))
 
     def _cross_kv(self, xa, st8, B):
         d = self.dims
@@ -393,22 +398,24 @@ class CudaEngine:
         return ses
 
     def _steps_descriptor(self, ses):
-        """Arguments of the persistent small-batch decode kernel (wts_decode_steps): float32 weights + this session's
-        caches, token state and scratch.  None when the model's dimensions are outside what the kernel supports."""
+        """Arguments of the lean small-batch decode step (wts_decode_step_kernels): SB16 weights + this session's caches,
+        token state and scratch.  None when the model's dimensions or the device are outside what the kernels support
+        (those sessions decode every step with the per-operator graph)."""
         d, w, dev = self.dims, self.w, self.dev
         D, H, L, V = d.n_text_state, d.n_text_head, d.n_text_layer, d.n_vocab
         if D % 128 != 0 or D > 1280 or D != 64 * H:
+            return None
+        # one CTA per SM, and a CTA keeps at most two 8-feature tasks of the K = 4 D matrix-vector product (FC2)
+        if D // 8 > 2 * torch.cuda.get_device_properties(dev).multi_processor_count:
             return None
         st8, cap = ses["st8"], ses["cap"]
         layers = (nat.DecLayer * L)()
         for li, blk in enumerate(w.dec):
             a, c, y = blk.attn, blk.cross, layers[li]
-            y.ln1_g, y.ln1_b, y.w_qkv, y.b_qkv = a.ln_g.data_ptr(), a.ln_b.data_ptr(), a.qkv_f32.data_ptr(), a.qkv_b.data_ptr()
-            y.w_o, y.b_o = a.out_f32.data_ptr(), a.out_b.data_ptr()
-            y.ln2_g, y.ln2_b, y.w_cq, y.b_cq = c.ln_g.data_ptr(), c.ln_b.data_ptr(), c.q_f32.data_ptr(), c.q_b.data_ptr()
-            y.w_co, y.b_co = c.out_f32.data_ptr(), c.out_b.data_ptr()
+            y.ln1_g, y.ln1_b, y.b_qkv, y.b_o = a.ln_g.data_ptr(), a.ln_b.data_ptr(), a.qkv_b.data_ptr(), a.out_b.data_ptr()
+            y.ln2_g, y.ln2_b, y.b_cq, y.b_co = c.ln_g.data_ptr(), c.ln_b.data_ptr(), c.q_b.data_ptr(), c.out_b.data_ptr()
             y.ln3_g, y.ln3_b = blk.mlp_ln_g.data_ptr(), blk.mlp_ln_b.data_ptr()
-            y.w_fc1, y.b_fc1, y.w_fc2, y.b_fc2 = blk.fc1_f32.data_ptr(), blk.fc1_b.data_ptr(), blk.fc2_f32.data_ptr(), blk.fc2_b.data_ptr()
+            y.b_fc1, y.b_fc2 = blk.fc1_b.data_ptr(), blk.fc2_b.data_ptr()
             y.self_k, y.self_v = st8["sk"][li].data_ptr(), st8["sv"][li].data_ptr()
             y.cross_k16, y.cross_v16 = st8["ck"][li].data_ptr(), st8["cv"][li].data_ptr()
             y.cross_k_align, y.head_slot = st8["ckal"][li].data_ptr(), w.head_slot[li].data_ptr()
@@ -419,8 +426,7 @@ class CudaEngine:
         raw = np.frombuffer(bytes(layers), dtype=np.uint8).copy()
         f32 = dict(dtype=torch.float32, device=dev)
         keep = dict(layers=torch.from_numpy(raw).to(dev), x=torch.zeros((cap, D), **f32), qkv=torch.zeros((cap, 3 * D), **f32),
-                    att=torch.zeros((cap, D), **f32), q=torch.zeros((cap, D), **f32), mid=torch.zeros((cap, 4 * D), **f32),
-                    sync=torch.zeros(64, dtype=torch.int32, device=dev))
+                    att=torch.zeros((cap, D), **f32), q=torch.zeros((cap, D), **f32), mid=torch.zeros((cap, 4 * D), **f32))
         p = nat.DecodeSteps()
         p.layers = keep["layers"].data_ptr()
         p.emb, p.pos, p.ln_g, p.ln_b = w.emb.data_ptr(), w.dec_pos.data_ptr(), w.ln_g.data_ptr(), w.ln_b.data_ptr()
@@ -430,78 +436,118 @@ class CudaEngine:
         p.last_full = ses["last_full"].data_ptr()
         p.suppress, p.blank = ses["suppress"].data_ptr(), ses["blank"].data_ptr()
         p.x, p.qkv, p.att, p.q, p.mid = (keep[k].data_ptr() for k in ("x", "qkv", "att", "q", "mid"))
-        p.logits, p.sync = ses["logits"].data_ptr(), keep["sync"].data_ptr()
+        p.logits = ses["logits"].data_ptr()
         p.emb_sb, p.emb_plane = w.emb_sb.ptr, w.emb_sb.plane
-        p.use_mma = 1 if self.small_batch_mma else 0
         p.cfg = ses["cfg"]
         p.n_layer, p.D, p.H, p.n_ctx, p.n_audio_ctx = L, D, H, d.n_text_ctx, N_CTX_AUDIO
         p.n_slots, p.cap, p.lp_ld, p.qk_rows = max(1, len(self.m.heads)), cap, ses["qk_rows"], ses["qk_rows"]
         return dict(args=p, keep=keep, host_layers=layers, graphs={})
 
-    def _lean_graph(self, ses, n_active):
-        """CUDA graph of ONE decoder step as the chain of lean per-phase kernels (wts_decode_step_kernels), for the
-        rows-per-pass variant that fits `n_active` (4 / 8 / 16 / 32 rows); captured on first use."""
-        sd = ses["steps"]
-        rows = 4 if n_active <= 4 else 8 if n_active <= 8 else 16 if n_active <= 16 else 32
-        key = (rows, bool(self.small_batch_mma))
-        if key in sd["graphs"]:
-            return sd["graphs"][key]
+    def _capture(self, ses, run):
+        """CUDA graph of `run()`, one decode step.  Every kernel must have run once outside capture (lazy module loading
+        and cudaFuncSetAttribute are not capturable), so `run()` is called once first on the live token state, which is
+        restored afterwards: that call is not a decode step of the caller.  The capture itself runs nothing."""
         dev = self.dev
-        p = sd["args"]
-
-        def launch():
-            p.max_rows, p.n_steps, p.use_mma = rows, 1, int(key[1])
-            nat.check(nat.lib.wts_decode_step_kernels(ctypes.byref(p), ctypes.byref(sd["host_layers"]), self._st()),
-                      "wts_decode_step_kernels")
         saved = {k: ses[k].clone() for k in ("tokens", "n_tokens", "done", "logprobs")}
-        launch()                                   # warm-up outside capture (module loading, function attributes) ...
-        torch.cuda.synchronize(dev)
-        for k, v in saved.items():                 # ... undone: it is not a decode step of the caller
-            ses[k].copy_(v)
-        graph = torch.cuda.CUDAGraph()
-        cap_stream = torch.cuda.Stream(device=dev)
-        cap_stream.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(cap_stream):
-            with torch.cuda.graph(graph, stream=cap_stream):
-                launch()
-        torch.cuda.current_stream(dev).wait_stream(cap_stream)
-        sd["graphs"][key] = graph
-        return graph
-
-    def _step_graph(self, ses):
-        """ONE captured CUDA graph of a per-operator decode step (captured on first use; the capture itself runs no
-        step — the warm-up call before it is NOT a decode step of the caller: it is undone by restoring the state)."""
-        if ses["graph"] is not None:
-            return ses["graph"]
-        dev = self.dev
-        # warm-up outside capture on a scratch copy of the token state (every kernel must have run once: lazy module
-        # loading and cudaFuncSetAttribute are not capturable)
-        saved = {k: ses[k].clone() for k in ("tokens", "n_tokens", "done", "logprobs")}
-        self._step(ses)
+        run()
         torch.cuda.synchronize(dev)
         for k, v in saved.items():
             ses[k].copy_(v)
         graph = torch.cuda.CUDAGraph()
         cap_stream = torch.cuda.Stream(device=dev)
         cap_stream.wait_stream(torch.cuda.current_stream(dev))
-        l0 = self.launches
         with torch.cuda.stream(cap_stream):
             with torch.cuda.graph(graph, stream=cap_stream):
-                self._step(ses)      # recorded, not executed
-        ses["per_step"] = self.launches - l0
-        self.launches = l0
+                run()
         torch.cuda.current_stream(dev).wait_stream(cap_stream)
-        ses["graph"] = graph
         return graph
 
-    def _run_steps(self, ses, n_steps, n_active):
-        """Up to n_steps decoder steps for the (<= small_batch_rows) sequences still decoding, in ONE cooperative
-        launch.  Returns nothing; the caller polls `done`."""
+    def _lean_graph(self, ses, n_active):
+        """CUDA graph of ONE decoder step as the chain of lean per-phase kernels (wts_decode_step_kernels), with grids
+        sized for 4 / 8 / 16 / 32 active rows, the smallest that fits `n_active`; captured on first use."""
         sd = ses["steps"]
-        p = sd["args"]
-        p.n_steps, p.max_rows = int(n_steps), int(n_active)
-        nat.check(nat.lib.wts_decode_steps(ctypes.byref(p), self._st()), "wts_decode_steps")
-        self.launches += 1
+        rows = 4 if n_active <= 4 else 8 if n_active <= 8 else 16 if n_active <= 16 else 32
+        if rows not in sd["graphs"]:
+            p = sd["args"]
+
+            def launch():
+                p.max_rows = rows
+                nat.check(nat.lib.wts_decode_step_kernels(ctypes.byref(p), ctypes.byref(sd["host_layers"]), self._st()),
+                          "wts_decode_step_kernels")
+            sd["graphs"][rows] = self._capture(ses, launch)
+        return sd["graphs"][rows]
+
+    def _step_graph(self, ses):
+        """ONE captured CUDA graph of a per-operator decode step (captured on first use)."""
+        if ses["graph"] is None:
+            l0 = self.launches
+            ses["graph"] = self._capture(ses, lambda: self._step(ses))
+            ses["per_step"] = (self.launches - l0) // 2       # the warm-up step and the recorded one
+            self.launches -= ses["per_step"]
+        return ses["graph"]
+
+    def _decode_chunk(self, ses, n_active, chunk, max_steps):
+        """`chunk` decode steps of every slot still decoding: the lean small-batch graph when at most `small_batch_rows`
+        windows are left, else the per-operator step (one graph, or plain launches for short decodes)."""
+        if ses["steps"] is not None and n_active <= self.small_batch_rows:
+            graph = self._lean_graph(ses, n_active)
+            for _ in range(chunk):
+                graph.replay()
+            self.launches += chunk * (8 * self.dims.n_text_layer + 3)
+            self.small_batch_steps += chunk
+        else:
+            graph = self._step_graph(ses) if (self.use_graph and max_steps > 4) else None
+            for _ in range(chunk):
+                if graph is not None:
+                    graph.replay()
+                    self.launches += ses["per_step"]
+                else:
+                    self._step(ses)
+        self.decode_steps_run += chunk
+
+    def _set_masks(self, ses, setup):
+        """Token masks of the logit filters: suppressed tokens, and the tokens blanked at the first sampled position."""
+        dev = self.dev
+        ses["suppress"].zero_()
+        ses["suppress"][torch.as_tensor(list(setup.suppress_tokens), dtype=torch.long, device=dev)] = 1
+        ses["blank"].zero_()
+        if setup.blank_tokens:
+            ses["blank"][torch.as_tensor(list(setup.blank_tokens), dtype=torch.long, device=dev)] = 1
+
+    def _prefill(self, ses, prompts, slots, tok, qk_last):
+        """Every prompt token of every window in one ragged batch through the decoder (own activation buffers, the
+        session's caches), then the final logits of each prompt's last row and of its <|startoftranscript|> row, and the
+        <|nospeech|> probability at the latter.  slots: session slot of each prompt; qk_last: the last prompt row writes
+        alignment row 0 of the session's qk buffer.  Returns (logits [2 n, V]: last rows, then SOT rows; no_speech [n])."""
+        d, dev, st, w = self.dims, self.dev, self._st(), self.w
+        D, V = d.n_text_state, d.n_vocab
+        n = len(prompts)
+        P = [len(p) for p in prompts]
+        R0 = sum(P)
+        row_seq = _i32([b for b, p in zip(slots, prompts) for _ in p], dev)
+        row_pos = _i32([i for p in prompts for i in range(len(p))], dev)
+        row_tok = _i32([t for p in prompts for t in p], dev)
+        qk_row = _i32([0 if qk_last and i == len(p) - 1 else -1 for p in prompts for i in range(len(p))], dev)
+        f32 = dict(dtype=torch.float32, device=dev)
+        pre = dict(ses["st8"])
+        pre.update(hs=SB16(R0, D, dev), att=SB16(R0, D, dev), mid=SB16(R0, 4 * D, dev),
+                   qkv=torch.empty((R0, 3 * D), **f32), q=torch.empty((R0, D), **f32))
+        x = torch.empty((R0, D), **f32)
+        nat.check(nat.lib.wts_embed(row_tok.data_ptr(), row_pos.data_ptr(), w.emb.data_ptr(), w.dec_pos.data_ptr(), R0, D,
+                                    x.data_ptr(), st), "wts_embed")
+        self._decoder_rows(pre, x, R0, row_seq, row_pos, qk_row, ses["qk_buf"])
+        ends = np.cumsum(P) - 1
+        sot_rows = [int(ends[k] - P[k] + 1 + prompts[k].index(tok.sot)) for k in range(n)]
+        sel = _i32(list(ends) + sot_rows, dev)
+        xr = torch.empty((2 * n, D), **f32)
+        nat.check(nat.lib.wts_gather_rows(x.data_ptr(), D, sel.data_ptr(), 2 * n, D, xr.data_ptr(), st), "wts_gather_rows")
+        logits2 = torch.empty((2 * n, V), **f32)
+        self._final_logits(xr, 2 * n, logits2)
+        no_speech = torch.zeros(n, **f32)
+        if tok.no_speech is not None:
+            nat.check(nat.lib.wts_softmax_pick(logits2.data_ptr() + 4 * n * V, V, V, tok.no_speech, no_speech.data_ptr(), n, st),
+                      "wts_softmax_pick")
+        return logits2, no_speech
 
     def _select(self, ses, logits, rows):
         d = self.dims
@@ -535,10 +581,9 @@ class CudaEngine:
 
     @torch.no_grad()
     def _decode_batch(self, jobs, setup):
-        d, dev, st, w = self.dims, self.dev, self._st(), self.w
+        d, dev = self.dims, self.dev
         tok = setup.tokenizer
         B = len(jobs)
-        D, V = d.n_text_state, d.n_vocab
         n_ctx = d.n_text_ctx
         sample_len = setup.sample_len
         ses = self._decoder_session(setup, B)
@@ -549,7 +594,6 @@ class CudaEngine:
             xa = self.encode(jobs)
         prompts = [list(j["prompt"]) for j in jobs]
         P = [len(p) for p in prompts]
-        R0 = sum(P)
         with self.phase("cross_kv"):
             self._cross_kv(xa, st8, B)
         del xa
@@ -567,83 +611,24 @@ class CudaEngine:
         dn[:B] = 0
         ses["done"].copy_(torch.from_numpy(dn))
         ses["logprobs"].zero_()
-        ses["suppress"].zero_()
-        ses["suppress"][torch.as_tensor(list(setup.suppress_tokens), dtype=torch.long, device=dev)] = 1
-        ses["blank"].zero_()
-        if setup.blank_tokens:
-            ses["blank"][torch.as_tensor(list(setup.blank_tokens), dtype=torch.long, device=dev)] = 1
+        self._set_masks(ses, setup)
         qk_buf = ses["qk_buf"]
 
-        # ---- prefill: every prompt token of every window in one ragged batch (own activation buffers)
-        row_seq = _i32([b for b, p in enumerate(prompts) for _ in p], dev)
-        row_pos = _i32([i for p in prompts for i in range(len(p))], dev)
-        row_tok = _i32([t for p in prompts for t in p], dev)
-        qk_row = _i32([0 if i == len(p) - 1 else -1 for p in prompts for i in range(len(p))], dev)
-        f32 = dict(dtype=torch.float32, device=dev)
-        pre = dict(st8)
-        pre.update(hs=SB16(R0, D, dev), att=SB16(R0, D, dev), mid=SB16(R0, 4 * D, dev),
-                   qkv=torch.empty((R0, 3 * D), **f32), q=torch.empty((R0, D), **f32))
-        x = torch.empty((R0, D), **f32)
-        ph = self.phase("prefill")
-        ph.__enter__()
-        nat.check(nat.lib.wts_embed(row_tok.data_ptr(), row_pos.data_ptr(), w.emb.data_ptr(), w.dec_pos.data_ptr(), R0, D,
-                                    x.data_ptr(), st), "wts_embed")
-        self._decoder_rows(pre, x, R0, row_seq, row_pos, qk_row, qk_buf)
-        ends = np.cumsum(P) - 1
-        sot_rows = [int(ends[b] - P[b] + 1 + prompts[b].index(tok.sot)) for b in range(B)]
-        sel = _i32(list(ends) + sot_rows, dev)
-        xr = torch.empty((2 * B, D), **f32)
-        nat.check(nat.lib.wts_gather_rows(x.data_ptr(), D, sel.data_ptr(), 2 * B, D, xr.data_ptr(), st), "wts_gather_rows")
-        logits2 = torch.empty((2 * B, V), **f32)
-        self._final_logits(xr, 2 * B, logits2)
-        no_speech = torch.zeros(B, **f32)
-        if tok.no_speech is not None:
-            nat.check(nat.lib.wts_softmax_pick(logits2.data_ptr() + 4 * B * V, V, V, tok.no_speech, no_speech.data_ptr(), B, st),
-                      "wts_softmax_pick")
-        self._select(ses, logits2, B)
-        ph.__exit__()
-        del pre, x, xr
+        with self.phase("prefill"):
+            logits2, no_speech = self._prefill(ses, prompts, range(B), tok, qk_last=True)
+            self._select(ses, logits2, B)
 
         # ---- decode steps
         max_steps = sample_len - 1
         steps_done = 0
-        ph = self.phase("decode_steps")
-        ph.__enter__()
         done = ses["done"]
         n_active = B
-        while steps_done < max_steps and n_active > 0:
-            left = max_steps - steps_done
-            if ses["steps"] is not None and n_active <= self.small_batch_rows and self.small_batch_mode == "lean":
-                # few sequences left: the lean per-phase kernels (float32 matrix-vector products, LayerNorm fused into the
-                # staging), one CUDA graph per step
-                chunk = min(8, left)
-                graph = self._lean_graph(ses, n_active)
-                for _ in range(chunk):
-                    graph.replay()
-                self.launches += chunk * (8 * d.n_text_layer + 3)
-                self.small_batch_steps += chunk
-            elif ses["steps"] is not None and n_active <= self.small_batch_rows:
-                # one persistent launch runs up to 32 whole steps (it stops by itself when all are done)
-                chunk = min(32, left)
-                self._run_steps(ses, chunk, n_active)
-                self.small_batch_steps += chunk
-            else:
-                chunk = min(8, left)
-                graph = self._step_graph(ses) if (self.use_graph and max_steps > 4) else None
-                for _ in range(chunk):
-                    if graph is not None:
-                        graph.replay()
-                        self.launches += ses["per_step"]
-                    else:
-                        self._step(ses)
-            steps_done += chunk
-            n_active = int((done == 0).sum().item())
-        if ses["steps"] is not None:
-            flags = ses["steps"]["keep"]["sync"].cpu().numpy()
-            if flags[1] != 0:
-                raise nat.WtsError("wts_decode_steps: grid barrier timed out (results invalid)")
-        ph.__exit__()
-        self.decode_steps_run = getattr(self, "decode_steps_run", 0) + steps_done
+        with self.phase("decode_steps"):
+            while steps_done < max_steps and n_active > 0:
+                chunk = min(8, max_steps - steps_done)
+                self._decode_chunk(ses, n_active, chunk, max_steps)
+                steps_done += chunk
+                n_active = int((done == 0).sum().item())
         if self.profile:
             self.batch_log = getattr(self, "batch_log", [])
             self.batch_log.append((B, steps_done, len(self._events) - 1))
@@ -694,22 +679,17 @@ class CudaEngine:
         slot while the other windows keep decoding.  The round-based `decode_windows` makes every round wait for its
         slowest window (a stuck one runs to the 224-token limit) before the follow-up windows even start.
         Same kernels, same per-window arithmetic as `decode_windows`; only the grouping of windows into steps differs."""
-        d, dev, st, w = self.dims, self.dev, self._st(), self.w
+        d, dev = self.dims, self.dev
         tok = setup.tokenizer
         assert not self.keep_full_logprobs, "decode_stream keeps no per-row log-prob tables"
-        D, V, n_ctx = d.n_text_state, d.n_vocab, d.n_text_ctx
+        n_ctx = d.n_text_ctx
         queue = list(jobs)
         if not queue:
             return
         ses = self._decoder_session(setup, min(self.max_batch, len(queue)))
         cap, st8, qk_buf = ses["cap"], ses["st8"], ses["qk_buf"]
-        f32 = dict(dtype=torch.float32, device=dev)
         ses["done"].fill_(1)
-        ses["suppress"].zero_()
-        ses["suppress"][torch.as_tensor(list(setup.suppress_tokens), dtype=torch.long, device=dev)] = 1
-        ses["blank"].zero_()
-        if setup.blank_tokens:
-            ses["blank"][torch.as_tensor(list(setup.blank_tokens), dtype=torch.long, device=dev)] = 1
+        self._set_masks(ses, setup)
         slot_job = [None] * cap               # job decoded in each slot
         slot_info = [None] * cap              # (prompt, no_speech_prob)
         free = list(range(cap))
@@ -735,7 +715,6 @@ class CudaEngine:
                 del xa
             prompts = [list(j["prompt"]) for _, j in batch]
             P = [len(p) for p in prompts]
-            R0 = sum(P)
             th = np.zeros((n, n_ctx + 1), dtype=np.int32)
             for k, p in enumerate(prompts):
                 th[k, :len(p)] = p
@@ -745,28 +724,7 @@ class CudaEngine:
             ses["n_prompt"].index_copy_(0, d_slots, nt)
             ses["logprobs"].index_fill_(0, d_slots, 0.0)
             with self.phase("prefill"):
-                row_seq = _i32([b for b, p in zip(slots, prompts) for _ in p], dev)
-                row_pos = _i32([i for p in prompts for i in range(len(p))], dev)
-                row_tok = _i32([t for p in prompts for t in p], dev)
-                qk_row = _i32([0 if i == len(p) - 1 else -1 for p in prompts for i in range(len(p))], dev)
-                pre = dict(st8)
-                pre.update(hs=SB16(R0, D, dev), att=SB16(R0, D, dev), mid=SB16(R0, 4 * D, dev),
-                           qkv=torch.empty((R0, 3 * D), **f32), q=torch.empty((R0, D), **f32))
-                x = torch.empty((R0, D), **f32)
-                nat.check(nat.lib.wts_embed(row_tok.data_ptr(), row_pos.data_ptr(), w.emb.data_ptr(), w.dec_pos.data_ptr(), R0, D,
-                                            x.data_ptr(), st), "wts_embed")
-                self._decoder_rows(pre, x, R0, row_seq, row_pos, qk_row, qk_buf)
-                ends = np.cumsum(P) - 1
-                sot_rows = [int(ends[k] - P[k] + 1 + prompts[k].index(tok.sot)) for k in range(n)]
-                sel = _i32(list(ends) + sot_rows, dev)
-                xr = torch.empty((2 * n, D), **f32)
-                nat.check(nat.lib.wts_gather_rows(x.data_ptr(), D, sel.data_ptr(), 2 * n, D, xr.data_ptr(), st), "wts_gather_rows")
-                logits2 = torch.empty((2 * n, V), **f32)
-                self._final_logits(xr, 2 * n, logits2)
-                no_speech = torch.zeros(n, **f32)
-                if tok.no_speech is not None:
-                    nat.check(nat.lib.wts_softmax_pick(logits2.data_ptr() + 4 * n * V, V, V, tok.no_speech, no_speech.data_ptr(), n, st),
-                              "wts_softmax_pick")
+                logits2, no_speech = self._prefill(ses, prompts, slots, tok, qk_last=True)
                 # first token of the new windows only: the select kernel works slot-wise, so the other slots are parked
                 ses["logits"].index_copy_(0, d_slots, logits2[:n])
                 saved = ses["done"].clone()
@@ -820,27 +778,10 @@ class CudaEngine:
                 while queue and free:
                     batch.append((free.pop(0), queue.pop(0)))
                 admit(batch)
-            ph = self.phase("decode_steps")
-            ph.__enter__()
-            n_active = int((done == 0).sum().item())
-            if n_active > 0:
-                chunk = 8
-                if ses["steps"] is not None and n_active <= self.small_batch_rows and self.small_batch_mode == "lean":
-                    graph = self._lean_graph(ses, n_active)
-                    for _ in range(chunk):
-                        graph.replay()
-                    self.launches += chunk * (8 * d.n_text_layer + 3)
-                    self.small_batch_steps += chunk
-                else:
-                    graph = self._step_graph(ses) if (self.use_graph and max_steps > 4) else None
-                    for _ in range(chunk):
-                        if graph is not None:
-                            graph.replay()
-                            self.launches += ses["per_step"]
-                        else:
-                            self._step(ses)
-                self.decode_steps_run = getattr(self, "decode_steps_run", 0) + chunk
-            ph.__exit__()
+            with self.phase("decode_steps"):
+                n_active = int((done == 0).sum().item())
+                if n_active > 0:
+                    self._decode_chunk(ses, n_active, 8, max_steps)
             done_h = done.cpu().numpy()
             finished = [b for b in range(cap) if slot_job[b] is not None and int(done_h[b]) != 0]
             if finished:
@@ -850,16 +791,6 @@ class CudaEngine:
                         queue.append(nxt)
                 free.extend(finished)
                 free.sort()
-
-    def _alloc_cross_state(self, B):
-        """Cross-attention K/V buffers for B windows (the layout of the session's, used as a staging area)."""
-        d, dev = self.dims, self.dev
-        H, L = d.n_text_head, d.n_text_layer
-        return dict(
-            ck=[torch.empty((B, H, N_CTX_AUDIO, 64), dtype=torch.float16, device=dev) for _ in range(L)],
-            cv=[torch.empty((B, H, N_CTX_AUDIO, 64), dtype=torch.float16, device=dev) for _ in range(L)],
-            ckal=[torch.empty((B, max(1, len(self.m.heads)), N_CTX_AUDIO, 64), dtype=torch.float32, device=dev) for _ in range(L)],
-            kvtmp=torch.empty((B, H, N_CTX_AUDIO, 64), dtype=torch.float32, device=dev))
 
     # ------------------------------------------------------------------ beam search / sampling (upstream strategies)
     @torch.no_grad()
@@ -873,14 +804,14 @@ class CudaEngine:
         bookkeeping is upstream's, on the host: top-(beam+1) candidates per row, de-duplicated per sequence, best
         beam_size kept, finished pool, patience; sampling draws from torch's global CPU generator exactly like the
         reference on CPU does (Categorical over the filtered rows).  KV-cache rows follow their source hypothesis."""
-        d, dev, st, w = self.dims, self.dev, self._st(), self.w
+        d, dev, st = self.dims, self.dev, self._st()
         tok = setup.tokenizer
         G = setup.n_group
         beam = setup.beam_size
         T = float(setup.temperature)
         ses = self._decoder_session(setup, G)
         cap, st8 = ses["cap"], ses["st8"]
-        D, V, L, n_ctx = d.n_text_state, d.n_vocab, d.n_text_layer, d.n_text_ctx
+        V, L, n_ctx = d.n_vocab, d.n_text_layer, d.n_text_ctx
         f32 = dict(dtype=torch.float32, device=dev)
         with self.phase("encoder"):
             xa = self.encode([job])
@@ -904,33 +835,10 @@ class CudaEngine:
         dn = np.ones(cap, dtype=np.int32)
         dn[:G] = 0
         ses["done"].copy_(torch.from_numpy(dn))
-        ses["suppress"].zero_()
-        ses["suppress"][torch.as_tensor(list(setup.suppress_tokens), dtype=torch.long, device=dev)] = 1
-        ses["blank"].zero_()
-        if setup.blank_tokens:
-            ses["blank"][torch.as_tensor(list(setup.blank_tokens), dtype=torch.long, device=dev)] = 1
+        self._set_masks(ses, setup)
         # ---- prefill of hypothesis 0, then its self-attention cache is shared out
         with self.phase("prefill"):
-            row_seq = _i32([0] * P, dev)
-            row_pos = _i32(list(range(P)), dev)
-            row_tok = _i32(prompt, dev)
-            qk_row = _i32([-1] * P, dev)
-            pre = dict(st8)
-            pre.update(hs=SB16(P, D, dev), att=SB16(P, D, dev), mid=SB16(P, 4 * D, dev),
-                       qkv=torch.empty((P, 3 * D), **f32), q=torch.empty((P, D), **f32))
-            x = torch.empty((P, D), **f32)
-            nat.check(nat.lib.wts_embed(row_tok.data_ptr(), row_pos.data_ptr(), w.emb.data_ptr(), w.dec_pos.data_ptr(), P, D,
-                                        x.data_ptr(), st), "wts_embed")
-            self._decoder_rows(pre, x, P, row_seq, row_pos, qk_row, ses["qk_buf"])
-            sel = _i32([P - 1, prompt.index(tok.sot)], dev)
-            xr = torch.empty((2, D), **f32)
-            nat.check(nat.lib.wts_gather_rows(x.data_ptr(), D, sel.data_ptr(), 2, D, xr.data_ptr(), st), "wts_gather_rows")
-            logits2 = torch.empty((2, V), **f32)
-            self._final_logits(xr, 2, logits2)
-            no_speech = torch.zeros(1, **f32)
-            if tok.no_speech is not None:
-                nat.check(nat.lib.wts_softmax_pick(logits2.data_ptr() + 4 * V, V, V, tok.no_speech, no_speech.data_ptr(), 1, st),
-                          "wts_softmax_pick")
+            logits2, no_speech = self._prefill(ses, [prompt], [0], tok, qk_last=False)
             for li in range(L):
                 for name in ("sk", "sv"):
                     t = st8[name][li]
@@ -938,7 +846,6 @@ class CudaEngine:
                         t[1:G, :, :P].copy_(t[0:1, :, :P].expand(G - 1, t.shape[1], P, t.shape[3]))
             ses["logits"][:G].copy_(logits2[0:1].expand(G, V))
             self.launches += 6
-        del pre, x, xr
         # ---- upstream's main loop
         lp_dev = torch.empty((cap, V), **f32)
         seqs = [list(prompt) for _ in range(G)]

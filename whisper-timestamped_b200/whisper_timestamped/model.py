@@ -108,7 +108,7 @@ class WhisperB200:
         w.conv2_b = g("encoder.conv2.bias")
         w.enc_pos = g("encoder.positional_embedding")
 
-        def attn_block(prefix, dm, n_head, cross, keep_f32=False):
+        def attn_block(prefix, dm, n_head, cross, decoder=False):
             scale = (dm // n_head) ** -0.25
             b = SimpleNamespace()
             b.ln_g, b.ln_b = g(prefix + "_ln.weight"), g(prefix + "_ln.bias")
@@ -116,39 +116,27 @@ class WhisperB200:
             k = g(prefix + ".key.weight") * scale
             v, vb = g(prefix + ".value.weight"), g(prefix + ".value.bias")
             zeros = torch.zeros_like(qb)
-            out_w = g(prefix + ".out.weight")
             if cross:
                 b.q, b.q_b = lin(q), qb
                 b.k = lin(k)
                 b.v, b.v_b = lin(v), vb
-                b.q_f32 = q.contiguous()
             else:
-                qkv = torch.cat([q, k, v], 0).contiguous()
-                b.qkv = lin(qkv)
+                b.qkv = lin(torch.cat([q, k, v], 0))
                 b.qkv_b = torch.cat([qb, zeros, vb]).contiguous()
-                if keep_f32:
-                    b.qkv_f32 = qkv
-                else:                       # encoder only: separate q|k and v projections (V is produced transposed)
+                if not decoder:             # encoder only: separate q|k and v projections (V is produced transposed)
                     b.qk = lin(torch.cat([q, k], 0))
                     b.qk_b = torch.cat([qb, zeros]).contiguous()
                     b.v, b.v_b = lin(v), vb
-            b.out, b.out_b = lin(out_w), g(prefix + ".out.bias")
-            if keep_f32:
-                b.out_f32 = out_w
+            b.out, b.out_b = lin(g(prefix + ".out.weight")), g(prefix + ".out.bias")
             return b
 
         def block(prefix, dm, n_head, cross):
-            # decoder blocks also keep their float32 weights: the persistent small-batch decode kernel
-            # (csrc/decode_steps.cu) streams them directly (4 bytes/parameter, like the hi + lo planes of SB16)
             blk = SimpleNamespace()
-            blk.attn = attn_block(prefix + ".attn", dm, n_head, False, keep_f32=cross)
-            blk.cross = attn_block(prefix + ".cross_attn", dm, n_head, True, keep_f32=True) if cross else None
+            blk.attn = attn_block(prefix + ".attn", dm, n_head, False, decoder=cross)
+            blk.cross = attn_block(prefix + ".cross_attn", dm, n_head, True) if cross else None
             blk.mlp_ln_g, blk.mlp_ln_b = g(prefix + ".mlp_ln.weight"), g(prefix + ".mlp_ln.bias")
-            fc1, fc2 = g(prefix + ".mlp.0.weight"), g(prefix + ".mlp.2.weight")
-            blk.fc1, blk.fc1_b = lin(fc1), g(prefix + ".mlp.0.bias")
-            blk.fc2, blk.fc2_b = lin(fc2), g(prefix + ".mlp.2.bias")
-            if cross:
-                blk.fc1_f32, blk.fc2_f32 = fc1, fc2
+            blk.fc1, blk.fc1_b = lin(g(prefix + ".mlp.0.weight")), g(prefix + ".mlp.0.bias")
+            blk.fc2, blk.fc2_b = lin(g(prefix + ".mlp.2.weight")), g(prefix + ".mlp.2.bias")
             return blk
 
         w.enc = [block(f"encoder.blocks.{i}", da, d.n_audio_head, False) for i in range(d.n_audio_layer)]
