@@ -74,6 +74,15 @@ int wts_attn_prep_batch(const float* d_qk, int32_t N, int32_t Tmax, int32_t Fmax
                         const WtsSegDesc* d_segs, int32_t nseg, int32_t max_T, int32_t max_F,
                         float* d_cost, void* stream);
 
+/* The same with the row kernel chosen: kernel 1 = one warp per token row walks the N heads in order; kernel 2 = one
+ * CTA per token row, its warps take disjoint head subsets and their sums are added in warp order (deterministic, but
+ * a different float32 summation order than kernel 1); kernel 0 = wts_attn_prep_batch's choice: kernel 2 when
+ * N >= WTS_PREP_HEADS_MIN_N, else kernel 1. */
+#define WTS_PREP_HEADS_MIN_N 32
+int wts_attn_prep_batch_kernel(const float* d_qk, int32_t N, int32_t Tmax, int32_t Fmax,
+                               const WtsSegDesc* d_segs, int32_t nseg, int32_t max_T, int32_t max_F,
+                               float* d_cost, int32_t kernel, void* stream);
+
 /*
  * Batched monotonic DTW — replaces dtw.dtw(weights, step_pattern=symmetric1) at T.py:1572-1581
  * and the jumps extraction at T.py:1648-1652.
@@ -223,6 +232,18 @@ int wts_cross_attention_f16(const float* d_q, int64_t ldq, const void* d_k16, co
                             const int32_t* d_row_seq, int32_t rows, int32_t H, void* d_out_sb16, int64_t ldo,
                             int64_t o_plane, float* d_qk_out, int32_t qk_rows, const int32_t* d_qk_row,
                             const int32_t* d_row_active, void* stream);
+/* Per-layer compacted float32 K copy.  The slots of the alignment heads are numbered layer-major, so the heads of one
+ * decoder layer hold the contiguous slots [align_s0, align_s0 + align_n) and the layer's float32 K copy is
+ * [B][align_n][ctx][64]: head h of window b sits at (b * align_n + head_slot[h] - align_s0).  The alignment buffer
+ * d_qk_out keeps every slot: [B][n_slots][qk_rows][ctx].  A layer without alignment heads passes align_n = 0 and no
+ * copy.  wts_cross_kv_pack / wts_cross_attention_f16 are these entries with align_s0 = 0, align_n = n_slots. */
+int wts_cross_kv_pack_layer(const float* d_src, void* d_dst16, float* d_dst_align, const int32_t* d_head_slot,
+                            int32_t align_s0, int32_t align_n, int32_t B, int32_t H, int32_t ctx, void* stream);
+int wts_cross_attention_f16_layer(const float* d_q, int64_t ldq, const void* d_k16, const void* d_v16,
+                                  const float* d_k_align, const int32_t* d_head_slot, int32_t n_slots, int32_t align_s0,
+                                  int32_t align_n, int32_t ctx, const int32_t* d_row_seq, int32_t rows, int32_t H,
+                                  void* d_out_sb16, int64_t ldo, int64_t o_plane, float* d_qk_out, int32_t qk_rows,
+                                  const int32_t* d_qk_row, const int32_t* d_row_active, void* stream);
 
 /* Scatter new self-attention K/V rows (float32 [rows, D]) into the head-major caches at (seq, position). */
 int wts_kv_append(const float* d_k, const float* d_v, int64_t ld, const int32_t* d_row_seq,
@@ -264,12 +285,13 @@ typedef struct WtsDecLayer {
     const float *ln3_g, *ln3_b, *b_fc1, *b_fc2;                      /* MLP */
     float *self_k, *self_v;                                          /* [cap, H, n_ctx, 64] float32 */
     const void *cross_k16, *cross_v16;                               /* [cap, H, n_audio_ctx, 64] fp16 */
-    const float* cross_k_align;                                      /* [cap, n_slots, n_audio_ctx, 64] float32 */
+    const float* cross_k_align;                                      /* [cap, align_n, n_audio_ctx, 64] float32 */
     const int32_t* head_slot;                                        /* [H]: alignment slot of each head or -1 */
     /* the six matrices as split-bf16 (SB16) planes [2][out][in] (hi plane at the pointer, lo plane `pl_*` ELEMENTS
      * further), row pitch = in */
     const void *sb_qkv, *sb_o, *sb_cq, *sb_co, *sb_fc1, *sb_fc2;
     int64_t pl_qkv, pl_o, pl_cq, pl_co, pl_fc1, pl_fc2;
+    int32_t align_s0, align_n;                                       /* this layer's slots [align_s0, align_s0 + align_n) */
 } WtsDecLayer;
 
 typedef struct WtsDecodeSteps {

@@ -43,7 +43,8 @@ def main():
         for name in ("ck", "cv"):
             t = ses["st8"][name][li]
             t.copy_((torch.randn(t.shape, device="cuda", generator=g) * 0.5).to(t.dtype))
-        ses["st8"]["ckal"][li].normal_(0, 0.5, generator=g)
+        if ses["st8"]["ckal"][li] is not None:          # layers without alignment heads have no float32 K copy
+            ses["st8"]["ckal"][li].normal_(0, 0.5, generator=g)
     ses["suppress"].zero_()
     ses["suppress"][tok.eot] = 1                 # keep every window alive for the whole probe
     ses["blank"].zero_()

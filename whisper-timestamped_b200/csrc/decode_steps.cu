@@ -113,7 +113,7 @@ __device__ __noinline__ void cross_attention_phase(const WtsDecodeSteps& P, cons
         const float* kal = nullptr;
         float* qk_dst = nullptr;
         if (slot >= 0) {
-            kal = Lr.cross_k_align + ((int64_t)row * P.n_slots + slot) * P.n_audio_ctx * 64;
+            kal = Lr.cross_k_align + ((int64_t)row * Lr.align_n + slot - Lr.align_s0) * P.n_audio_ctx * 64;
             const int qr = __ldcg(P.n_tokens + row) - __ldg(P.n_prompt + row);
             qk_dst = P.qk_buf + (((int64_t)row * P.n_slots + slot) * P.qk_rows + qr) * (int64_t)P.n_audio_ctx;
         }

@@ -294,14 +294,14 @@ decoder_attention_kernel(const int kind, const float* q, int64_t ldq, const floa
 // rows are the DTW input and must stay within 1e-3 of the reference); all other heads use fp16 K.
 __global__ void cross_kv_pack_kernel(const float* __restrict__ src, __half* __restrict__ dst16,
                                      float* __restrict__ dst_align, const int32_t* __restrict__ head_slot,
-                                     int n_slots, int H, int ctx)
+                                     int s0, int n_l, int H, int ctx)
 {
     const int bh = blockIdx.x;                      // b * H + h
     const int b = bh / H, h = bh - b * H;
     const float* s = src + (int64_t)bh * ctx * 64;
     __half* d = dst16 + (int64_t)bh * ctx * 64;
     const int slot = dst_align ? head_slot[h] : -1;
-    float* da = slot >= 0 ? dst_align + ((int64_t)b * n_slots + slot) * ctx * 64 : nullptr;
+    float* da = slot >= 0 ? dst_align + ((int64_t)b * n_l + slot - s0) * ctx * 64 : nullptr;
     for (int i = threadIdx.x; i < ctx * 64; i += blockDim.x) {
         const float v = s[i];
         d[i] = __float2half_rn(v);
@@ -316,7 +316,7 @@ __global__ void cross_kv_pack_kernel(const float* __restrict__ src, __half* __re
 __global__ void __launch_bounds__(CA_THREADS)
 cross_attention_f16_kernel(const float* q, int64_t ldq, const __half* k16,
                            const __half* v16, const float* k_align,
-                           const int32_t* head_slot, int n_slots, int ctx,
+                           const int32_t* head_slot, int n_slots, int s0, int n_l, int ctx,
                            const int32_t* row_seq, int H, __nv_bfloat16* o, int64_t ldo,
                            int64_t o_plane, float* qk_out, int qk_rows, const int32_t* qk_row,
                            const int32_t* row_active)
@@ -339,7 +339,7 @@ cross_attention_f16_kernel(const float* q, int64_t ldq, const __half* k16,
     float* qk_dst = nullptr;
     const float* kal = nullptr;
     if (slot >= 0) {
-        kal = k_align + ((int64_t)seq * n_slots + slot) * ctx * 64;
+        kal = k_align + ((int64_t)seq * n_l + slot - s0) * ctx * 64;
         if (qk_out != nullptr) {
             const int qr = qk_row[r];
             if (qr >= 0) qk_dst = qk_out + (((int64_t)seq * n_slots + slot) * qk_rows + qr) * (int64_t)ctx;
@@ -572,12 +572,36 @@ extern "C" int wts_decoder_attention(int32_t kind, const float* d_q, int64_t ldq
 }
 
 
-extern "C" int wts_cross_kv_pack(const float* d_src, void* d_dst16, float* d_dst_align, const int32_t* d_head_slot,
-                                 int32_t n_slots, int32_t B, int32_t H, int32_t ctx, void* stream)
+extern "C" int wts_cross_kv_pack_layer(const float* d_src, void* d_dst16, float* d_dst_align,
+                                       const int32_t* d_head_slot, int32_t align_s0, int32_t align_n, int32_t B,
+                                       int32_t H, int32_t ctx, void* stream)
 {
     if (B <= 0) return 0;
     cross_kv_pack_kernel<<<B * H, 256, 0, (cudaStream_t)stream>>>(d_src, (__half*)d_dst16, d_dst_align, d_head_slot,
-                                                                 n_slots, H, ctx);
+                                                                 align_s0, align_n, H, ctx);
+    WTS_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" int wts_cross_kv_pack(const float* d_src, void* d_dst16, float* d_dst_align, const int32_t* d_head_slot,
+                                 int32_t n_slots, int32_t B, int32_t H, int32_t ctx, void* stream)
+{
+    return wts_cross_kv_pack_layer(d_src, d_dst16, d_dst_align, d_head_slot, 0, n_slots, B, H, ctx, stream);
+}
+
+extern "C" int wts_cross_attention_f16_layer(const float* d_q, int64_t ldq, const void* d_k16, const void* d_v16,
+                                             const float* d_k_align, const int32_t* d_head_slot, int32_t n_slots,
+                                             int32_t align_s0, int32_t align_n, int32_t ctx, const int32_t* d_row_seq,
+                                             int32_t rows, int32_t H, void* d_out_sb16, int64_t ldo, int64_t o_plane,
+                                             float* d_qk_out, int32_t qk_rows, const int32_t* d_qk_row,
+                                             const int32_t* d_row_active, void* stream)
+{
+    if (rows <= 0) return 0;
+    if ((ldq & 3) || (reinterpret_cast<uintptr_t>(d_q) & 15)) { set_error("wts_cross_attention_f16: q must be 16-byte aligned"); return -2; }
+    dim3 grid(rows, H);
+    WTS_CUDA_CHECK(launch_pdl(cross_attention_f16_kernel, grid, dim3(CA_THREADS), 0, (cudaStream_t)stream, 
+        d_q, ldq, (const __half*)d_k16, (const __half*)d_v16, d_k_align, d_head_slot, n_slots, align_s0, align_n, ctx,
+        d_row_seq, H, (__nv_bfloat16*)d_out_sb16, ldo, o_plane, d_qk_out, qk_rows, d_qk_row, d_row_active));
     WTS_LAUNCH_CHECK();
     return 0;
 }
@@ -589,14 +613,9 @@ extern "C" int wts_cross_attention_f16(const float* d_q, int64_t ldq, const void
                                        int32_t qk_rows, const int32_t* d_qk_row, const int32_t* d_row_active,
                                        void* stream)
 {
-    if (rows <= 0) return 0;
-    if ((ldq & 3) || (reinterpret_cast<uintptr_t>(d_q) & 15)) { set_error("wts_cross_attention_f16: q must be 16-byte aligned"); return -2; }
-    dim3 grid(rows, H);
-    WTS_CUDA_CHECK(launch_pdl(cross_attention_f16_kernel, grid, dim3(CA_THREADS), 0, (cudaStream_t)stream, 
-        d_q, ldq, (const __half*)d_k16, (const __half*)d_v16, d_k_align, d_head_slot, n_slots, ctx, d_row_seq, H,
-        (__nv_bfloat16*)d_out_sb16, ldo, o_plane, d_qk_out, qk_rows, d_qk_row, d_row_active));
-    WTS_LAUNCH_CHECK();
-    return 0;
+    return wts_cross_attention_f16_layer(d_q, ldq, d_k16, d_v16, d_k_align, d_head_slot, n_slots, 0, n_slots, ctx,
+                                         d_row_seq, rows, H, d_out_sb16, ldo, o_plane, d_qk_out, qk_rows, d_qk_row,
+                                         d_row_active, stream);
 }
 
 extern "C" int wts_kv_append(const float* d_k, const float* d_v, int64_t ld, const int32_t* d_row_seq,

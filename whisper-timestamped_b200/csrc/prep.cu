@@ -26,6 +26,54 @@ namespace wts {
 
 constexpr int PREP_WARPS = 4;
 
+// One head of one token row, by one warp: slice -> median of 9 -> softmax, added to acc[] (first head: stored).
+__device__ __forceinline__ void prep_head_row(const float* __restrict__ src, const int F, const int lane, float* xb,
+                                              float* mbuf, float* acc, const bool first)
+{
+    const int npair = (F + 1) >> 1;
+    for (int c = lane; c < F; c += 32) xb[c + 4] = __ldg(src + c);
+    __syncwarp();
+    if (lane < 4) {                                   // scipy 'reflect' halo (periodic for tiny F)
+        xb[3 - lane] = xb[4 + wts_reflect_index(-1 - lane, F)];
+        xb[F + 4 + lane] = xb[4 + wts_reflect_index(F + lane, F)];
+    }
+    if (lane == 4) xb[F + 8] = 0.f;
+    __syncwarp();
+    float mx = -INFINITY;
+    for (int p = lane; p < npair; p += 32) {
+        const int c = 2 * p;
+        float v[10];
+        const float2* x2 = reinterpret_cast<const float2*>(xb + c);
+#pragma unroll
+        for (int k = 0; k < 5; ++k) { const float2 q = x2[k]; v[2 * k] = q.x; v[2 * k + 1] = q.y; }
+        float m0, m1;
+        wts_median9_pair(v, &m0, &m1);
+        mbuf[c] = m0;
+        mx = fmaxf(mx, m0);
+        if (c + 1 < F) { mbuf[c + 1] = m1; mx = fmaxf(mx, m1); }
+    }
+    mx = warp_max(mx);
+    float sum = 0.f;
+    for (int c = lane; c < F; c += 32) {
+        const float e = __expf(mbuf[c] - mx);
+        mbuf[c] = e;
+        sum += e;
+    }
+    sum = warp_sum(sum);
+    const float inv = 1.0f / sum;
+    if (first) { for (int c = lane; c < F; c += 32) acc[c] = mbuf[c] * inv; }
+    else       { for (int c = lane; c < F; c += 32) acc[c] += mbuf[c] * inv; }
+    __syncwarp();
+}
+
+__device__ __forceinline__ const float* prep_row_src(const float* qk, const WtsSegDesc& sd, const int t, const int N,
+                                                     const int Tmax, const int Fmax)
+{
+    const int row = (t == sd.T - 1) ? sd.last_row : sd.row0 + t;
+    return qk + (((int64_t)sd.window * N) * Tmax + row) * (int64_t)Fmax + sd.f0;
+}
+
+// Serial over heads: one warp per (segment, token) row walks all N heads.
 __global__ void __launch_bounds__(PREP_WARPS * 32)
 prep_rows_kernel(const float* __restrict__ qk, const int N, const int Tmax, const int Fmax,
                  const WtsSegDesc* __restrict__ segs, const int pitch, float* __restrict__ cost)
@@ -40,51 +88,48 @@ prep_rows_kernel(const float* __restrict__ qk, const int N, const int Tmax, cons
     float* mbuf = xb + pitch;                        // median-filtered -> exp
     float* acc = mbuf + pitch;                       // sum over heads of the softmax rows
 
-    const int row = (t == sd.T - 1) ? sd.last_row : sd.row0 + t;
-    const float* src0 = qk + (((int64_t)sd.window * N) * Tmax + row) * (int64_t)Fmax + sd.f0;
+    const float* src0 = prep_row_src(qk, sd, t, N, Tmax, Fmax);
     const int64_t head_stride = (int64_t)Tmax * Fmax;
-    const int npair = (F + 1) >> 1;
-
-    for (int n = 0; n < N; ++n) {
-        const float* src = src0 + n * head_stride;
-        for (int c = lane; c < F; c += 32) xb[c + 4] = __ldg(src + c);
-        __syncwarp();
-        if (lane < 4) {                               // scipy 'reflect' halo (periodic for tiny F)
-            xb[3 - lane] = xb[4 + wts_reflect_index(-1 - lane, F)];
-            xb[F + 4 + lane] = xb[4 + wts_reflect_index(F + lane, F)];
-        }
-        if (lane == 4) xb[F + 8] = 0.f;
-        __syncwarp();
-        float mx = -INFINITY;
-        for (int p = lane; p < npair; p += 32) {
-            const int c = 2 * p;
-            float v[10];
-            const float2* x2 = reinterpret_cast<const float2*>(xb + c);
-#pragma unroll
-            for (int k = 0; k < 5; ++k) { const float2 q = x2[k]; v[2 * k] = q.x; v[2 * k + 1] = q.y; }
-            float m0, m1;
-            wts_median9_pair(v, &m0, &m1);
-            mbuf[c] = m0;
-            mx = fmaxf(mx, m0);
-            if (c + 1 < F) { mbuf[c + 1] = m1; mx = fmaxf(mx, m1); }
-        }
-        mx = warp_max(mx);
-        float sum = 0.f;
-        for (int c = lane; c < F; c += 32) {
-            const float e = __expf(mbuf[c] - mx);
-            mbuf[c] = e;
-            sum += e;
-        }
-        sum = warp_sum(sum);
-        const float inv = 1.0f / sum;
-        if (n == 0) { for (int c = lane; c < F; c += 32) acc[c] = mbuf[c] * inv; }
-        else        { for (int c = lane; c < F; c += 32) acc[c] += mbuf[c] * inv; }
-        __syncwarp();
-    }
+    for (int n = 0; n < N; ++n) prep_head_row(src0 + n * head_stride, F, lane, xb, mbuf, acc, n == 0);
     const int P = seg_pitch(sd);
     float* dst = cost + sd.cost_off + (int64_t)t * P;
     const float fn = (float)N;
     for (int c = lane; c < P; c += 32) dst[c] = c < F ? acc[c] / fn : 0.f;     // padding columns (pitch) hold zeros
+}
+
+// Head-parallel: one CTA per (segment, token) row; warp w takes heads w, w + PREP_WARPS, ... into its own shared row,
+// then the CTA adds the warps' rows in warp order (fixed order: the result does not depend on timing).  For the
+// many-head sets (every head of the top layers: 100-320 heads), where the serial walk is 10-30x the work per row.
+__global__ void __launch_bounds__(PREP_WARPS * 32)
+prep_rows_heads_kernel(const float* __restrict__ qk, const int N, const int Tmax, const int Fmax,
+                       const WtsSegDesc* __restrict__ segs, const int pitch, float* __restrict__ cost)
+{
+    extern __shared__ float smem[];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const WtsSegDesc sd = segs[blockIdx.x];
+    const int t = blockIdx.y;
+    if (t >= sd.T) return;                           // whole CTA: no barrier is skipped by part of it
+    const int F = sd.F;
+    float* xb = smem + (size_t)warp * 3 * pitch;
+    float* mbuf = xb + pitch;
+    float* acc = mbuf + pitch;
+    const float* src0 = prep_row_src(qk, sd, t, N, Tmax, Fmax);
+    const int64_t head_stride = (int64_t)Tmax * Fmax;
+    for (int n = warp; n < N; n += PREP_WARPS) prep_head_row(src0 + n * head_stride, F, lane, xb, mbuf, acc, n == warp);
+    __syncthreads();
+    const int nw = min(N, PREP_WARPS);
+    const int P = seg_pitch(sd);
+    float* dst = cost + sd.cost_off + (int64_t)t * P;
+    const float fn = (float)N;
+    for (int c = threadIdx.x; c < P; c += blockDim.x) {
+        float s = 0.f;
+        if (c < F) {
+            s = smem[2 * pitch + c];
+            for (int w = 1; w < nw; ++w) s += smem[(size_t)w * 3 * pitch + 2 * pitch + c];
+            s /= fn;
+        }
+        dst[c] = s;
+    }
 }
 
 __global__ void __launch_bounds__(256)
@@ -154,9 +199,9 @@ extern "C" int wts_disfluency_starts(const float* d_cost, const WtsSegDesc* d_se
     return 0;
 }
 
-extern "C" int wts_attn_prep_batch(const float* d_qk, int32_t N, int32_t Tmax, int32_t Fmax,
-                                   const WtsSegDesc* d_segs, int32_t nseg, int32_t max_T,
-                                   int32_t max_F, float* d_cost, void* stream)
+extern "C" int wts_attn_prep_batch_kernel(const float* d_qk, int32_t N, int32_t Tmax, int32_t Fmax,
+                                          const WtsSegDesc* d_segs, int32_t nseg, int32_t max_T, int32_t max_F,
+                                          float* d_cost, int32_t kernel, void* stream)
 {
     if (nseg <= 0) return 0;
     if (!d_qk || !d_segs || !d_cost) { set_error("wts_attn_prep_batch: null pointer"); return -2; }
@@ -164,15 +209,31 @@ extern "C" int wts_attn_prep_batch(const float* d_qk, int32_t N, int32_t Tmax, i
         set_error("wts_attn_prep_batch: bad geometry N=%d max_T=%d max_F=%d Fmax=%d", N, max_T, max_F, Fmax);
         return -2;
     }
+    if (kernel < 0 || kernel > 2) { set_error("wts_attn_prep_batch_kernel: kernel %d is not 0, 1 or 2", kernel); return -2; }
+    if (kernel == 0) kernel = N >= WTS_PREP_HEADS_MIN_N ? 2 : 1;
     cudaStream_t st = (cudaStream_t)stream;
     const int pitch = (max_F + 10 + 1) & ~1;            // halo + even pitch so float2 reads stay aligned
     const size_t smem = (size_t)PREP_WARPS * 3 * pitch * sizeof(float);
-    if (smem > 48 * 1024)
-        WTS_CUDA_CHECK(cudaFuncSetAttribute(prep_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    dim3 grid(nseg, (max_T + PREP_WARPS - 1) / PREP_WARPS);
-    prep_rows_kernel<<<grid, PREP_WARPS * 32, smem, st>>>(d_qk, N, Tmax, Fmax, d_segs, pitch, d_cost);
+    if (kernel == 1) {
+        if (smem > 48 * 1024)
+            WTS_CUDA_CHECK(cudaFuncSetAttribute(prep_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        dim3 grid(nseg, (max_T + PREP_WARPS - 1) / PREP_WARPS);
+        prep_rows_kernel<<<grid, PREP_WARPS * 32, smem, st>>>(d_qk, N, Tmax, Fmax, d_segs, pitch, d_cost);
+    } else {
+        if (smem > 48 * 1024)
+            WTS_CUDA_CHECK(cudaFuncSetAttribute(prep_rows_heads_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        dim3 grid(nseg, max_T);
+        prep_rows_heads_kernel<<<grid, PREP_WARPS * 32, smem, st>>>(d_qk, N, Tmax, Fmax, d_segs, pitch, d_cost);
+    }
     WTS_LAUNCH_CHECK();
     prep_cols_kernel<<<nseg, 256, 0, st>>>(d_segs, d_cost);
     WTS_LAUNCH_CHECK();
     return 0;
+}
+
+extern "C" int wts_attn_prep_batch(const float* d_qk, int32_t N, int32_t Tmax, int32_t Fmax,
+                                   const WtsSegDesc* d_segs, int32_t nseg, int32_t max_T,
+                                   int32_t max_F, float* d_cost, void* stream)
+{
+    return wts_attn_prep_batch_kernel(d_qk, N, Tmax, Fmax, d_segs, nseg, max_T, max_F, d_cost, 0, stream);
 }

@@ -66,7 +66,7 @@ class DecLayer(ctypes.Structure):
         "ln1_g", "ln1_b", "b_qkv", "b_o", "ln2_g", "ln2_b", "b_cq", "b_co", "ln3_g", "ln3_b", "b_fc1", "b_fc2",
         "self_k", "self_v", "cross_k16", "cross_v16", "cross_k_align", "head_slot",
         "sb_qkv", "sb_o", "sb_cq", "sb_co", "sb_fc1", "sb_fc2")] + [(n, ctypes.c_int64) for n in (
-        "pl_qkv", "pl_o", "pl_cq", "pl_co", "pl_fc1", "pl_fc2")]
+        "pl_qkv", "pl_o", "pl_cq", "pl_co", "pl_fc1", "pl_fc2")] + [("align_s0", ctypes.c_int32), ("align_n", ctypes.c_int32)]
 
 
 class DecodeSteps(ctypes.Structure):
@@ -94,6 +94,8 @@ def _load():
     vp, i32 = ctypes.c_void_p, ctypes.c_int32
     lib.wts_attn_prep_batch.restype = ctypes.c_int
     lib.wts_attn_prep_batch.argtypes = [vp, i32, i32, i32, vp, i32, i32, i32, vp, vp]
+    lib.wts_attn_prep_batch_kernel.restype = ctypes.c_int
+    lib.wts_attn_prep_batch_kernel.argtypes = [vp, i32, i32, i32, vp, i32, i32, i32, vp, i32, vp]
     lib.wts_dtw_batch.restype = ctypes.c_int
     lib.wts_dtw_batch.argtypes = [vp, i32, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp]
     lib.wts_dtw_batch_sized.restype = ctypes.c_int
@@ -117,6 +119,9 @@ def _load():
                                           i32, vp, vp, vp]
     lib.wts_cross_kv_pack.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, vp]
     lib.wts_cross_attention_f16.argtypes = [vp, i64, vp, vp, vp, vp, i32, i32, vp, i32, i32, vp, i64, i64, vp, i32, vp, vp, vp]
+    lib.wts_cross_kv_pack_layer.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]
+    lib.wts_cross_attention_f16_layer.argtypes = [vp, i64, vp, vp, vp, vp, i32, i32, i32, i32, vp, i32, i32, vp, i64, i64,
+                                                  vp, i32, vp, vp, vp]
     lib.wts_enc_attention.argtypes = [vp, i64, i64, vp, i64, i64, i32, i32, i32, i32, vp, i64, i64, vp]
     lib.wts_enc_attention.restype = ctypes.c_int
     lib.wts_kv_append.argtypes = [vp, vp, i64, vp, vp, i32, i32, i32, vp, vp, i64, vp]
@@ -131,7 +136,7 @@ def _load():
     for name in ("wts_to_sb16", "wts_layernorm", "wts_softmax_rows", "wts_frames", "wts_power", "wts_logmel_max",
                  "wts_logmel_finish", "wts_window_gather", "wts_embed", "wts_gather_rows", "wts_decoder_attention",
                  "wts_kv_append", "wts_decode_select", "wts_step_inputs", "wts_softmax_pick", "wts_logprob_gather", "wts_cross_kv_pack",
-                 "wts_cross_attention_f16"):
+                 "wts_cross_attention_f16", "wts_cross_kv_pack_layer", "wts_cross_attention_f16_layer"):
         getattr(lib, name).restype = ctypes.c_int
     return lib
 
@@ -144,6 +149,7 @@ EXPORTED_SYMBOLS = [
     "wts_frames", "wts_power", "wts_logmel_max", "wts_logmel_finish", "wts_window_gather", "wts_embed",
     "wts_gather_rows", "wts_decoder_attention", "wts_kv_append", "wts_decode_select", "wts_filtered_logprobs", "wts_decode_step_kernels", "wts_step_inputs",
     "wts_softmax_pick", "wts_logprob_gather", "wts_cross_kv_pack", "wts_cross_attention_f16", "wts_enc_attention",
+    "wts_cross_kv_pack_layer", "wts_cross_attention_f16_layer", "wts_attn_prep_batch_kernel",
 ]
 
 

@@ -95,8 +95,9 @@ def _segs_to_device(arr: np.ndarray, device) -> torch.Tensor:
 
 
 def attn_prep(qk: torch.Tensor, plan: AlignPlan, cost: torch.Tensor = None,
-              d_segs: torch.Tensor = None) -> torch.Tensor:
-    """qk: float32 [n_windows, N, Tmax, Fmax] on the GPU.  Returns the float32 cost buffer."""
+              d_segs: torch.Tensor = None, kernel: int = 0) -> torch.Tensor:
+    """qk: float32 [n_windows, N, Tmax, Fmax] on the GPU.  Returns the float32 cost buffer.
+    kernel: 0 = chosen by N, 1 = serial over heads, 2 = head-parallel (wts_attn_prep_batch_kernel)."""
     nat.require_cuda(qk, "qk")
     assert qk.dtype == torch.float32 and qk.dim() == 4 and qk.is_contiguous()
     _, N, Tmax, Fmax = qk.shape
@@ -104,9 +105,9 @@ def attn_prep(qk: torch.Tensor, plan: AlignPlan, cost: torch.Tensor = None,
         cost = torch.empty(plan.cost_elems, dtype=torch.float32, device=qk.device)
     if d_segs is None:
         d_segs = _segs_to_device(plan.segs, qk.device)
-    rc = nat.lib.wts_attn_prep_batch(nat.ptr(qk), N, Tmax, Fmax, nat.ptr(d_segs), plan.nseg,
-                                     plan.max_T, plan.max_F, nat.ptr(cost), nat.stream_ptr(qk.device))
-    nat.check(rc, "wts_attn_prep_batch")
+    rc = nat.lib.wts_attn_prep_batch_kernel(nat.ptr(qk), N, Tmax, Fmax, nat.ptr(d_segs), plan.nseg, plan.max_T,
+                                            plan.max_F, nat.ptr(cost), kernel, nat.stream_ptr(qk.device))
+    nat.check(rc, "wts_attn_prep_batch_kernel")
     return cost
 
 

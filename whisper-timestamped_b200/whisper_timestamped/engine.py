@@ -59,6 +59,31 @@ class CudaEngine:
         self._graphs = {}
         self.profile = False            # when set, phases are bracketed with CUDA events (stage_ms())
         self._events = []
+        self.heads = None
+        self.set_alignment_heads(model.heads)
+
+    # ------------------------------------------------------------------ alignment heads
+    def set_alignment_heads(self, heads=None):
+        """Heads whose cross-attention rows the decoder exports for word alignment, as (layer, head) pairs (None: the
+        model's own heads); they get slots in layer-major order, so the heads of layer l hold the contiguous slots
+        [s0_l, s0_l + n_l).  The slot tables, the per-layer float32 K copies and the decode session (and its CUDA
+        graphs) are rebuilt only when the set changes."""
+        heads = sorted((int(l), int(h)) for l, h in (self.m.heads if heads is None else heads))
+        if heads == self.heads:
+            return
+        d = self.dims
+        L, H = d.n_text_layer, d.n_text_head
+        assert heads and all(0 <= l < L and 0 <= h < H for l, h in heads), heads
+        assert len(set(heads)) == len(heads), "duplicate alignment heads"
+        slots = torch.full((L, H), -1, dtype=torch.int32)
+        for s_, (l, h) in enumerate(heads):
+            slots[l, h] = s_
+        self.heads = heads
+        self.head_slot = slots.to(self.dev)
+        counts = [sum(1 for l, _ in heads if l == li) for li in range(L)]
+        self.layer_slots = [(sum(counts[:li]), counts[li]) for li in range(L)]      # (s0_l, n_l)
+        self._session = None
+        self._tf_state = None
 
     # ------------------------------------------------------------------ phase timers
     class _Phase:
@@ -260,9 +285,11 @@ class CudaEngine:
         d, w, st = self.dims, self.w, self._st()
         D, H, L = d.n_text_state, d.n_text_head, d.n_text_layer
         hs, qkv, att, q, mid = st8["hs"], st8["qkv"], st8["att"], st8["q"], st8["mid"]
-        n_slots = len(self.m.heads)
+        n_slots = len(self.heads)
         for li, blk in enumerate(w.dec):
             a, c = blk.attn, blk.cross
+            s0, n_l = self.layer_slots[li]
+            kal = st8["ckal"][li]
             self.layernorm(x, a.ln_g, a.ln_b, R, D, out_sb=hs)
             self.gemm(hs, a.qkv, R, 3 * D, D, bias=a.qkv_b, out_f32=qkv, ldc=3 * D, row_mask=active)
             fused_append = active is not None          # decode step: one row per sequence, the attention CTA appends K/V
@@ -280,12 +307,11 @@ class CudaEngine:
             self.gemm(att, a.out, R, D, D, bias=a.out_b, residual=x, ldr=D, out_f32=x, ldc=D, row_mask=active)
             self.layernorm(x, c.ln_g, c.ln_b, R, D, out_sb=hs)
             self.gemm(hs, c.q, R, D, D, bias=c.q_b, out_f32=q, ldc=D, row_mask=active)
-            nat.check(nat.lib.wts_cross_attention_f16(q.data_ptr(), D, st8["ck"][li].data_ptr(), st8["cv"][li].data_ptr(),
-                                                      st8["ckal"][li].data_ptr(), w.head_slot[li].data_ptr(), n_slots,
-                                                      N_CTX_AUDIO, row_seq.data_ptr(), R, H, att.ptr, att.ld, att.plane,
-                                                      qk_buf.data_ptr(), qk_buf.shape[2], qk_row.data_ptr(),
-                                                      active.data_ptr() if active is not None else None, st),
-                      "wts_cross_attention_f16")
+            nat.check(nat.lib.wts_cross_attention_f16_layer(
+                q.data_ptr(), D, st8["ck"][li].data_ptr(), st8["cv"][li].data_ptr(), kal.data_ptr() if kal is not None else None,
+                self.head_slot[li].data_ptr(), n_slots, s0, n_l, N_CTX_AUDIO, row_seq.data_ptr(), R, H, att.ptr, att.ld,
+                att.plane, qk_buf.data_ptr(), qk_buf.shape[2], qk_row.data_ptr(),
+                active.data_ptr() if active is not None else None, st), "wts_cross_attention_f16_layer")
             self.gemm(att, c.out, R, D, D, bias=c.out_b, residual=x, ldr=D, out_f32=x, ldc=D, row_mask=active)
             self.layernorm(x, blk.mlp_ln_g, blk.mlp_ln_b, R, D, out_sb=hs)
             self.gemm(hs, blk.fc1, R, 4 * D, D, bias=blk.fc1_b, act=1, out_sb=mid, row_mask=active)
@@ -312,7 +338,9 @@ class CudaEngine:
         return dict(
             ck=[torch.empty((B, H, N_CTX_AUDIO, 64), dtype=torch.float16, device=dev) for _ in range(L)],
             cv=[torch.empty((B, H, N_CTX_AUDIO, 64), dtype=torch.float16, device=dev) for _ in range(L)],
-            ckal=[torch.empty((B, max(1, len(self.m.heads)), N_CTX_AUDIO, 64), dtype=torch.float32, device=dev) for _ in range(L)],
+            # float32 K of each layer's own alignment heads only (none: no buffer)
+            ckal=[torch.empty((B, n_l, N_CTX_AUDIO, 64), dtype=torch.float32, device=dev) if n_l else None
+                  for (_, n_l) in self.layer_slots],
             kvtmp=torch.empty((B, H, N_CTX_AUDIO, 64), dtype=torch.float32, device=dev))
 
     def _cross_kv(self, xa, st8, B):
@@ -321,13 +349,14 @@ class CudaEngine:
         for li, blk in enumerate(self.w.dec):
             c = blk.cross
             tmp = st8["kvtmp"]
-            n_slots = len(self.m.heads)
+            s0, n_l = self.layer_slots[li]
             for (wt, bias, dst, al) in ((c.k, None, st8["ck"][li], st8["ckal"][li]), (c.v, c.v_b, st8["cv"][li], None)):
                 self.gemm(xa, wt, 1500, D, D, batch=(B, 1), a_b=(1500 * D, 0), bias=bias, out_f32=tmp, ldc=64,
                           c_b=(H * 1500 * 64, 0), head_dim=64, head_stride=1500 * 64)
-                nat.check(nat.lib.wts_cross_kv_pack(tmp.data_ptr(), dst.data_ptr(), al.data_ptr() if al is not None else None,
-                                                    self.w.head_slot[li].data_ptr(), n_slots, B, H, N_CTX_AUDIO, self._st()),
-                          "wts_cross_kv_pack")
+                nat.check(nat.lib.wts_cross_kv_pack_layer(tmp.data_ptr(), dst.data_ptr(),
+                                                          al.data_ptr() if al is not None else None,
+                                                          self.head_slot[li].data_ptr(), s0, n_l, B, H, N_CTX_AUDIO,
+                                                          self._st()), "wts_cross_kv_pack_layer")
                 self.launches += 1
 
     def _final_logits(self, x_rows, n_rows, logits):
@@ -343,9 +372,40 @@ class CudaEngine:
             # upstream decoding strategies (beam search / best-of-n sampling): one window at a time, n_group hypotheses
             return [self._decode_strategy(job, setup) for job in jobs]
         out = []
-        for i in range(0, len(jobs), self.max_batch):
-            out.extend(self._decode_batch(jobs[i:i + self.max_batch], setup))
+        limit = self.batch_limit(setup)
+        for i in range(0, len(jobs), limit):
+            out.extend(self._decode_batch(jobs[i:i + limit], setup))
         return out
+
+    def window_bytes(self, sample_len):
+        """Device bytes one window of a decode batch needs: its slot of the decode session (cross K/V, float32 K of the
+        alignment heads, self-attention caches, alignment rows and the buffer they are collected into) and the encoder
+        activations of the window."""
+        d = self.dims
+        L, H, D, n_ctx = d.n_text_layer, d.n_text_head, d.n_text_state, d.n_text_ctx
+        N, ctx = len(self.heads), N_CTX_AUDIO
+        cross = L * H * ctx * 64 * 2 * 2 + N * ctx * 64 * 4 + H * ctx * 64 * 4
+        self_kv = 2 * L * H * n_ctx * 64 * 4
+        rows = 2 * N * (sample_len + 1) * ctx * 4
+        Da = d.n_audio_state
+        encoder = 3002 * d.n_mels * 4 + 3001 * Da * 4 + ctx * Da * (4 + 4 + 8 + 4 + 16 + 4) + Da * KPAD * 4
+        return cross + self_kv + rows + encoder
+
+    def batch_limit(self, setup):
+        """Windows per decode batch: WTS_MAX_BATCH (default 64), lowered when that many windows of this head set
+        would not fit in 85 % of the device memory that is free when the first batch of the head set is sized (torch's
+        unused cached blocks are returned first: fragments of them cannot hold a session's multi-GB buffers)."""
+        key = (tuple(self.heads), setup.sample_len)
+        lim = getattr(self, "_limits", {})
+        if key not in lim:
+            torch.cuda.empty_cache()
+            free, _ = torch.cuda.mem_get_info(self.dev)
+            ses = getattr(self, "_session", None)
+            if ses is not None:                                    # the session of the same head set is reused
+                free += ses["cap"] * self.window_bytes(setup.sample_len)
+            lim[key] = max(1, min(self.max_batch, int(0.85 * free) // self.window_bytes(setup.sample_len)))
+            self._limits = lim
+        return lim[key]
 
     def _decoder_session(self, setup, need):
         """Persistent decode state for up to `max_batch` windows: KV caches, token buffers, the alignment buffer
@@ -358,7 +418,7 @@ class CudaEngine:
         cap = 4
         while cap < need:
             cap *= 2
-        cap = min(cap, max(self.max_batch, need))
+        cap = min(cap, max(self.batch_limit(setup), need))
         if ses is not None and ses["cap"] >= need:
             cap = ses["cap"]                      # a smaller batch reuses the larger session (and its graph)
         key = (cap, setup.sample_len, tok.eot, tok.timestamp_begin, tok.no_timestamps, setup.max_initial_timestamp_index,
@@ -367,7 +427,7 @@ class CudaEngine:
             return ses
         self._session = ses = None
         qk_rows = setup.sample_len + 1
-        n_slots = len(self.m.heads)
+        n_slots = len(self.heads)
         i32 = dict(dtype=torch.int32, device=dev)
         ses = dict(key=key, cap=cap, qk_rows=qk_rows, graph=None, per_step=0)
         ses["st8"] = self._alloc_decoder_state(cap, cap)
@@ -379,6 +439,10 @@ class CudaEngine:
         ses["logprobs"] = torch.zeros((cap, qk_rows), dtype=torch.float32, device=dev)
         ses["full"] = torch.empty((cap, qk_rows, V), dtype=torch.float32, device=dev) if self.keep_full_logprobs else None
         ses["qk_buf"] = torch.zeros((cap, max(1, n_slots), qk_rows, N_CTX_AUDIO), dtype=torch.float32, device=dev)
+        # a batch's alignment rows are collected here (allocated once: no multi-GB allocation per batch); while an
+        # earlier batch's rows still occupy it (not yet aligned and freed), a batch gets a copy of its own
+        ses["qk_out"] = torch.zeros_like(ses["qk_buf"])
+        ses["qk_out_idx"] = None
         ses["s_tok"] = torch.zeros(cap, **i32)
         ses["s_pos"] = torch.zeros(cap, **i32)
         ses["s_qkr"] = torch.zeros(cap, **i32)
@@ -418,7 +482,9 @@ class CudaEngine:
             y.b_fc1, y.b_fc2 = blk.fc1_b.data_ptr(), blk.fc2_b.data_ptr()
             y.self_k, y.self_v = st8["sk"][li].data_ptr(), st8["sv"][li].data_ptr()
             y.cross_k16, y.cross_v16 = st8["ck"][li].data_ptr(), st8["cv"][li].data_ptr()
-            y.cross_k_align, y.head_slot = st8["ckal"][li].data_ptr(), w.head_slot[li].data_ptr()
+            kal = st8["ckal"][li]
+            y.cross_k_align, y.head_slot = kal.data_ptr() if kal is not None else None, self.head_slot[li].data_ptr()
+            y.align_s0, y.align_n = self.layer_slots[li]
             for name, sb in (("qkv", a.qkv), ("o", a.out), ("cq", c.q), ("co", c.out), ("fc1", blk.fc1), ("fc2", blk.fc2)):
                 assert sb.ld == sb.cols
                 setattr(y, "sb_" + name, sb.ptr)
@@ -440,7 +506,7 @@ class CudaEngine:
         p.emb_sb, p.emb_plane = w.emb_sb.ptr, w.emb_sb.plane
         p.cfg = ses["cfg"]
         p.n_layer, p.D, p.H, p.n_ctx, p.n_audio_ctx = L, D, H, d.n_text_ctx, N_CTX_AUDIO
-        p.n_slots, p.cap, p.lp_ld, p.qk_rows = max(1, len(self.m.heads)), cap, ses["qk_rows"], ses["qk_rows"]
+        p.n_slots, p.cap, p.lp_ld, p.qk_rows = len(self.heads), cap, ses["qk_rows"], ses["qk_rows"]
         return dict(args=p, keep=keep, host_layers=layers, graphs={})
 
     def _capture(self, ses, run):
@@ -641,7 +707,14 @@ class CudaEngine:
         ns_h = no_speech.cpu().numpy()
         max_rows = int(max(1, (n_tok_h - np.asarray(P)).max() + 1))
         buf_idx = len(self.qk_buffers)
-        self.qk_buffers.append(qk_buf[:B, :, :max_rows].clone())     # the session buffer is reused by the next batch
+        i = ses["qk_out_idx"]                                         # the session buffer is reused by the next batch
+        if i is None or i >= len(self.qk_buffers) or self.qk_buffers[i] is None:
+            rows = ses["qk_out"][:B]
+            rows[:, :, :max_rows].copy_(qk_buf[:B, :, :max_rows])
+            ses["qk_out_idx"] = buf_idx
+        else:
+            rows = qk_buf[:B, :, :max_rows].clone()
+        self.qk_buffers.append(rows)
         full = ses["full"]
         if full is not None:
             self.full_logprobs.append(full[:B, :max_rows].clone())
@@ -672,13 +745,14 @@ class CudaEngine:
 
     # ------------------------------------------------------------------ continuous batching
     @torch.no_grad()
-    def decode_stream(self, jobs, setup, feed):
+    def decode_stream(self, jobs, setup, feed, collected=None):
         """Greedy decoding with CONTINUOUS batching: decode `jobs`; as soon as a window finishes its record goes to
         `feed(job, record)`, which may return the next window of that audio stream (upstream's seek loop: the follow-up
         window of a 30-s cut, or the next window of a long file) — it is encoded, prefilled and admitted into the freed
         slot while the other windows keep decoding.  The round-based `decode_windows` makes every round wait for its
         slowest window (a stuck one runs to the 224-token limit) before the follow-up windows even start.
-        Same kernels, same per-window arithmetic as `decode_windows`; only the grouping of windows into steps differs."""
+        Same kernels, same per-window arithmetic as `decode_windows`; only the grouping of windows into steps differs.
+        `collected()`, when given, is called after the records of each collection have been fed."""
         d, dev = self.dims, self.dev
         tok = setup.tokenizer
         assert not self.keep_full_logprobs, "decode_stream keeps no per-row log-prob tables"
@@ -686,7 +760,7 @@ class CudaEngine:
         queue = list(jobs)
         if not queue:
             return
-        ses = self._decoder_session(setup, min(self.max_batch, len(queue)))
+        ses = self._decoder_session(setup, min(self.batch_limit(setup), len(queue)))
         cap, st8, qk_buf = ses["cap"], ses["st8"], ses["qk_buf"]
         ses["done"].fill_(1)
         self._set_masks(ses, setup)
@@ -710,7 +784,8 @@ class CudaEngine:
                     self._cross_kv(xa, tmp, n)
                     for li in range(d.n_text_layer):
                         for name in ("ck", "cv", "ckal"):
-                            st8[name][li].index_copy_(0, d_slots, tmp[name][li])
+                            if st8[name][li] is not None:
+                                st8[name][li].index_copy_(0, d_slots, tmp[name][li])
                     del tmp
                 del xa
             prompts = [list(j["prompt"]) for _, j in batch]
@@ -789,6 +864,8 @@ class CudaEngine:
                     nxt = feed(job, rec)
                     if nxt is not None:
                         queue.append(nxt)
+                if collected is not None:
+                    collected()
                 free.extend(finished)
                 free.sort()
 
@@ -820,7 +897,7 @@ class CudaEngine:
             for li in range(L):                          # every hypothesis attends to the same audio
                 for name in ("ck", "cv", "ckal"):
                     t = st8[name][li]
-                    if G > 1:
+                    if G > 1 and t is not None:
                         t[1:G].copy_(t[0:1].expand(G - 1, *t.shape[1:]))
         del xa
         prompt = list(job["prompt"])
@@ -968,7 +1045,7 @@ class CudaEngine:
             self._cross_kv(xa, st8, 1)
         del xa
         rows = R - (i_start - 1)
-        qk_buf = torch.zeros((1, max(1, len(self.m.heads)), rows, N_CTX_AUDIO), dtype=torch.float32, device=dev)
+        qk_buf = torch.zeros((1, len(self.heads), rows, N_CTX_AUDIO), dtype=torch.float32, device=dev)
         row_seq = _i32([0] * R, dev)
         row_pos = _i32(list(range(R)), dev)
         row_tok = _i32(tokens_in, dev)
@@ -1013,7 +1090,7 @@ class CudaEngine:
         xa = self.encode([job])
         st8 = self._alloc_decoder_state(1, 1)
         self._cross_kv(xa, st8, 1)
-        qk_buf = torch.zeros((1, max(1, len(self.m.heads)), 1, N_CTX_AUDIO), dtype=torch.float32, device=dev)
+        qk_buf = torch.zeros((1, len(self.heads), 1, N_CTX_AUDIO), dtype=torch.float32, device=dev)
         x = torch.empty((1, d.n_text_state), dtype=torch.float32, device=dev)
         one = _i32([0], dev)
         t = _i32([tokenizer.sot], dev)
@@ -1062,6 +1139,12 @@ class CudaEngine:
                 for (i, _, _), l_ in zip(lst, split_jumps(dl.cpu().numpy(), plan)):
                     lefts[i] = l_[:-1]
         return (out, lefts) if disfluencies else out
+
+    def free_alignment_rows(self, windows):
+        """Drop the alignment rows of the decode batches holding these (already aligned) windows."""
+        for gid in windows:
+            if gid >= 0:
+                self.qk_buffers[self.window_index[gid][0]] = None
 
     def release(self):
         self.qk_buffers.clear()

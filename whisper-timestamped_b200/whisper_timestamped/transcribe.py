@@ -8,9 +8,9 @@ Same signature, option checks and return value as the reference
      decoded in ONE engine batch (encoder + greedy decoder on the GPU, cross-attention rows of the
      alignment heads written straight into the alignment buffer — no forward hooks, no per-token
      device->host copies: replaces T.py:783-793, 849-881);
-  2. when all windows are decoded, the hook state machine of the reference is replayed offline
-     (windows.py) to find the segments, and ALL segments are aligned in one batch on the GPU
-     (alignment.py: attention post-processing + DTW);
+  2. as soon as a decode batch is consumed, the hook state machine of the reference is replayed offline
+     (windows.py) on its windows to find the segments, and all of them are aligned in one batch on the GPU
+     (alignment.py: attention post-processing + DTW); the batch's alignment rows are then freed;
   3. words, confidences and post-processing follow T.py:912-1002 and 313-357.
 """
 import logging
@@ -89,6 +89,13 @@ class _Stream:
             self.all_tokens.extend(s["tokens"])
         if not condition_on_previous_text or rec.temperature > 0.5:
             self.prompt_reset_since = len(self.all_tokens)
+
+
+def top_layers_heads(n_layer, n_head, k):
+    """`word_alignment_most_top_layers=k`: every head of the top k decoder layers (k clipped at the number of layers),
+    layer-major — the order of the reference's reshape to [k*H, T, F] (T.py:1542-1543)."""
+    assert k > 0, "word_alignment_most_top_layers must be a strictly positive number"
+    return [(l, h) for l in range(max(0, n_layer - k), n_layer) for h in range(n_head)]
 
 
 def decode_with_fallback(eng, jobs, setup, temperatures, tokenizer, compression_ratio_threshold, logprob_threshold,
@@ -202,13 +209,18 @@ def transcribe_timestamped(
     if seed is not None:                   # T.py:223-225: sampling (temperature > 0) draws from torch's global generator
         import torch
         torch.manual_seed(seed)
-    if word_alignment_most_top_layers is not None:
-        raise NotImplementedError("word_alignment_most_top_layers: only the alignment-head tables are built")
 
     eng = engine if engine is not None else model.engine()
     if hasattr(eng, "release"):
-        eng.release()                      # alignment buffers of a previous call (they are per call, 1.7 GB per 128 windows)
+        eng.release()                      # alignment buffers of a previous call
     dims = model.dims
+    # alignment heads of this call: every head of the top k layers (T.py:259, 401, 892, 1542-1548), else the model's own
+    if word_alignment_most_top_layers is not None:
+        if not hasattr(eng, "set_alignment_heads"):
+            raise NotImplementedError("word_alignment_most_top_layers: this engine cannot change its alignment heads")
+        eng.set_alignment_heads(top_layers_heads(dims.n_text_layer, dims.n_text_head, word_alignment_most_top_layers))
+    elif hasattr(eng, "set_alignment_heads"):
+        eng.set_alignment_heads(None)
     is_multilingual = model.is_multilingual
     num_languages = model.num_languages
 
@@ -260,30 +272,93 @@ def transcribe_timestamped(
         content_frames = eng.mel_frames(mel) - N_FRAMES
         streams.append(_Stream(i, mel, content_frames, s / SAMPLE_RATE, initial_prompt_tokens))
 
+    use_space = should_use_space(language)
+    consumed = []         # (stream, window idx, prompt of the stream's next window or None) not yet aligned
+    aligned = {}          # (stream idx, window idx) -> (plans, info, [(plan, request, jumps, disfluency starts)])
+
+    def align_consumed():
+        """One-pass strategy: plan and align the windows consumed since the last call (one decode batch, or one
+        collection of continuous batching), then free their alignment rows.  A window's plan needs only its own tokens
+        and the next window's prompt, which consume() has produced; the jumps stay on the host until the words are
+        assembled at the end."""
+        if naive_approach or not consumed:
+            consumed.clear()
+            return
+        pending, items = [], []
+        for st, wi, nxt in consumed:
+            rec = st.records[wi]
+            reqs = {}
+
+            def yields_words(plan, reqs=reqs):
+                # T.py:540-559: `ws` is empty when there is nothing between the timestamps or every word is a
+                # special token; this only depends on the tokens, so it is known before the DTW runs
+                req = None
+                if len(plan.tokens) > 1:
+                    req = W.prepare_alignment(plan.tokens, plan.n_rows, tokenizer, use_space=use_space,
+                                              refine_nframes=refine_nframes,
+                                              remove_punctuation_from_words=remove_punctuation_from_words,
+                                              unfinished_decoding=plan.unfinished)
+                reqs[id(plan)] = req
+                if req is None:
+                    return False
+                kept = req.words[1:] if req.unfinished else req.words[1:-1]
+                return any(not w.startswith("<|") for w in kept)
+
+            plans, info = plan_window_alignment(rec, setup, nxt, yields_words)
+            aligned[(st.index, wi)] = (plans, info, [])
+            for plan in plans:
+                req = reqs[id(plan)]
+                for msg in (req.warnings if req is not None else []):
+                    logger.warning(msg)
+                if req is not None and rec.max_duration and req.f0 >= rec.max_duration:
+                    logger.warning("Got start time outside of audio boundary")
+                if req is None:
+                    aligned[(st.index, wi)][2].append((plan, None, None, None))
+                    continue
+                pending.append((st.index, wi, plan, req))
+                items.append(dict(window=rec.qk_window, row0=plan.row0, last_row=plan.row0 + req.row_offset_last,
+                                  T=req.T, f0=req.f0, F=req.F, max_dur=rec.max_duration or 0))
+        lefts_list = None
+        if items and detect_disfluencies:
+            jumps_list, lefts_list = eng.align(items, disfluencies=True)
+        else:
+            jumps_list = eng.align(items) if items else []
+        for (si, wi, plan, req), j, l_ in zip(pending, jumps_list, lefts_list or [None] * len(jumps_list)):
+            aligned[(si, wi)][2].append((plan, req, j, l_))
+        if hasattr(eng, "free_alignment_rows"):
+            eng.free_alignment_rows([st.records[wi].qk_window for st, wi, _ in consumed])
+        consumed.clear()
+
     # ---- decode: the next window of every active stream in one GPU batch
     def consume(job, rec):
         st = streams[job["stream"]]
         if language_detected and job["stream"] == 0 and not st.records:
             rec.mel_from_language_detection = True        # first window of the file, see WindowRecord.max_duration
         st.consume(rec, tokenizer, no_speech_threshold, logprob_threshold, condition_on_previous_text)
-        return st.next_job(setup) if st.active else None
+        nxt = st.next_job(setup) if st.active else None
+        consumed.append((st, len(st.records) - 1, nxt["prompt"] if nxt is not None else None))
+        return nxt
 
     plain_greedy = len(temperatures) == 1 and temperatures[0] == 0 and setup.beam_size is None
     if plain_greedy and hasattr(eng, "decode_stream") and continuous_batching:
         # continuous batching: a stream's next window is admitted into the decode batch as soon as its previous one
         # finishes (no round barrier); per stream the windows are still decoded strictly in upstream's order
-        eng.decode_stream([st.next_job(setup) for st in streams if st.active], setup, consume)
+        eng.decode_stream([st.next_job(setup) for st in streams if st.active], setup, consume, collected=align_consumed)
     else:
+        # one decode batch at a time (the engine's batch size), so that only one batch of alignment rows is alive
+        limit = eng.batch_limit(setup) if hasattr(eng, "batch_limit") and not naive_approach else None
         while True:
             jobs = [st.next_job(setup) for st in streams if st.active]
             if not jobs:
                 break
-            records = decode_with_fallback(eng, jobs, setup, temperatures, tokenizer, compression_ratio_threshold,
-                                           logprob_threshold, no_speech_threshold)
-            for job, rec in zip(jobs, records):
-                consume(job, rec)
-
-    use_space = should_use_space(language)
+            for i in range(0, len(jobs), limit or len(jobs)):
+                part = jobs[i:i + limit] if limit else jobs
+                records = decode_with_fallback(eng, part, setup, temperatures, tokenizer, compression_ratio_threshold,
+                                               logprob_threshold, no_speech_threshold)
+                for job, rec in zip(part, records):
+                    consume(job, rec)
+                align_consumed()
+    align_consumed()
     if naive_approach:
         # ---- two-pass strategy (T.py:1004-1338): pass 1 above was plain decoding; pass 2 re-runs the decoder teacher-forced
         # on every segment's own audio window and aligns all of its tokens at once
@@ -302,53 +377,6 @@ def transcribe_timestamped(
             w["_stream"] = 0
         text_parts = [tokenizer.decode(st.all_tokens[st.n_initial_prompt:])]
     else:
-        # ---- replay the reference's segment/flush logic offline and align everything in one batch
-        use_space = should_use_space(language)
-        pending = []          # (stream, window idx, plan, AlignRequest)
-        per_window = {}
-        for st in streams:
-            for wi, rec in enumerate(st.records):
-                nxt = st.records[wi + 1].prompt if wi + 1 < len(st.records) else None
-                reqs = {}
-
-                def yields_words(plan, reqs=reqs):
-                    # T.py:540-559: `ws` is empty when there is nothing between the timestamps or every word is a
-                    # special token; this only depends on the tokens, so it is known before the DTW runs
-                    req = None
-                    if len(plan.tokens) > 1:
-                        req = W.prepare_alignment(plan.tokens, plan.n_rows, tokenizer, use_space=use_space,
-                                                  refine_nframes=refine_nframes,
-                                                  remove_punctuation_from_words=remove_punctuation_from_words,
-                                                  unfinished_decoding=plan.unfinished)
-                    reqs[id(plan)] = req
-                    if req is None:
-                        return False
-                    kept = req.words[1:] if req.unfinished else req.words[1:-1]
-                    return any(not w.startswith("<|") for w in kept)
-
-                plans, info = plan_window_alignment(rec, setup, nxt, yields_words)
-                per_window[(st.index, wi)] = (plans, info)
-                for plan in plans:
-                    req = reqs[id(plan)]
-                    for msg in req.warnings:
-                        logger.warning(msg)
-                    if rec.max_duration and req.f0 >= rec.max_duration:
-                        logger.warning("Got start time outside of audio boundary")
-                    pending.append((st, wi, plan, req))
-        items = []
-        for (st, wi, plan, req) in pending:
-            if req is None:
-                continue
-            rec = st.records[wi]
-            items.append(dict(window=rec.qk_window, row0=plan.row0, last_row=plan.row0 + req.row_offset_last,
-                              T=req.T, f0=req.f0, F=req.F, max_dur=rec.max_duration or 0))
-        lefts_list = None
-        if items and detect_disfluencies:
-            jumps_list, lefts_list = eng.align(items, disfluencies=True)
-        else:
-            jumps_list = eng.align(items) if items else []
-        jit = iter(zip(jumps_list, lefts_list if lefts_list is not None else [None] * len(jumps_list)))
-
         # ---- per stream: words, confidences, compile (T.py:712-771, 912-1002)
         all_segments, all_words = [], []
         text_parts = []
@@ -357,15 +385,11 @@ def transcribe_timestamped(
             seg_logprobs = []     # log-probs of the text tokens of the same segments
             seg_avglogprob = []
             seg_tokens = []       # the token list each flushed segment ended up with
-            pend_iter = [p for p in pending if p[0] is st]
-            by_window = {}
-            for p in pend_iter:
-                by_window.setdefault(p[1], []).append(p)
             for wi, rec in enumerate(st.records):
-                plans, info = per_window[(st.index, wi)]
+                plans, info, done = aligned[(st.index, wi)]
                 ws_of_window, kept_plans = [], []
-                for (_, _, plan, req) in by_window.get(wi, []):
-                    ws = W.words_from_jumps(req, *next(jit), tokenizer=tokenizer) if req is not None else []
+                for (plan, req, jumps, lefts) in done:
+                    ws = W.words_from_jumps(req, jumps, lefts, tokenizer=tokenizer) if req is not None else []
                     assert ws, "plan_window_alignment only keeps segments that yield words"
                     ws_of_window.append(ws)
                     kept_plans.append(plan)
