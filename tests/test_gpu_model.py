@@ -396,3 +396,37 @@ def test_continuous_batching_equals_rounds():
             wx, wy = x.get("words", []), y.get("words", [])
             assert [(w_["text"], w_["start"], w_["end"]) for w_ in wx] == [(w_["text"], w_["start"], w_["end"]) for w_ in wy]
             assert all(abs(p["confidence"] - q["confidence"]) <= 2e-3 for p, q in zip(wx, wy))
+
+
+def test_alignment_rows_held_across_collections():
+    """Alignment rows nobody has freed stay intact while later windows are decoded: only the first collection of
+    decode_stream (and the first batch of decode_windows) gets the session's row buffer, every later one keeps a copy
+    of its own.  Every window is aligned at the very end, and both paths give the same jumps."""
+    import whisper_timestamped as wt
+    from whisper_timestamped.engine import CudaEngine
+    from whisper_timestamped.synthetic_audio import synthetic_speech
+    from whisper_timestamped.tokenizer import get_tokenizer
+    from whisper_timestamped.windows import make_decode_setup
+    gm = wt.load_model("synthetic:tiny", device="cuda:0")
+    tok = get_tokenizer(True, num_languages=gm.num_languages, language="en", task="transcribe")
+    setup = make_decode_setup(tok, gm.dims.n_text_ctx)
+    audio = synthetic_speech(200.0, seed=51)
+
+    def aligned(eng, recs):
+        qk_out = eng._session["qk_out"].data_ptr()
+        assert [b.data_ptr() == qk_out for b in eng.qk_buffers] == [True] + [False] * (len(eng.qk_buffers) - 1)
+        items = [dict(window=r.qk_window, row0=0, last_row=r.n_rows - 1, T=r.n_rows, f0=0, F=1500, max_dur=0) for r in recs]
+        return eng.align(items)
+
+    stream = CudaEngine(gm, max_batch=4)
+    mel = stream.log_mel(stream.load_audio(audio))
+    jobs = [dict(mel=mel, seek=s, segment_size=3000, prompt=setup.initial_tokens([])) for s in range(0, 20000, 2000)]
+    got = {}
+    stream.decode_stream(jobs, setup, lambda job, rec: got.__setitem__(job["seek"], rec))
+    a = [got[j["seek"]] for j in jobs]
+    rounds = CudaEngine(gm, max_batch=4)
+    b = rounds.decode_windows(jobs, setup)
+    assert len(stream.qk_buffers) > 2 and len(rounds.qk_buffers) == 3
+    for k, (x, y, jx, jy) in enumerate(zip(a, b, aligned(stream, a), aligned(rounds, b))):
+        assert x.tokens == y.tokens and x.n_rows == y.n_rows, k
+        assert np.array_equal(jx, jy), k

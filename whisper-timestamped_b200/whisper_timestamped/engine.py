@@ -359,13 +359,15 @@ class CudaEngine:
                                                           self._st()), "wts_cross_kv_pack_layer")
                 self.launches += 1
 
-    def _final_logits(self, x_rows, n_rows, logits):
-        """LN + tied-embedding projection of `n_rows` float32 rows -> logits [n_rows, V]."""
+    def _final_logits(self, x_rows, n_rows, logits, hs=None, row_mask=None):
+        """LN + tied-embedding projection of `n_rows` float32 rows -> logits [n_rows, V].  hs: the SB16 LN output (a
+        fresh one when None; the decode step passes its own so that a captured graph allocates nothing)."""
         d, w = self.dims, self.w
         D, V = d.n_text_state, d.n_vocab
-        hs = SB16(n_rows, D, self.dev)
+        if hs is None:
+            hs = SB16(n_rows, D, self.dev)
         self.layernorm(x_rows, w.ln_g, w.ln_b, n_rows, D, out_sb=hs)
-        self.gemm(hs, w.emb_sb, n_rows, V, D, out_f32=logits, ldc=V)
+        self.gemm(hs, w.emb_sb, n_rows, V, D, out_f32=logits, ldc=V, row_mask=row_mask)
 
     def decode_windows(self, jobs, setup):
         if getattr(setup, "beam_size", None) is not None or setup.temperature > 0:
@@ -437,10 +439,12 @@ class CudaEngine:
         ses["n_prompt"] = torch.ones(cap, **i32)
         ses["done"] = torch.ones(cap, **i32)
         ses["logprobs"] = torch.zeros((cap, qk_rows), dtype=torch.float32, device=dev)
+        ses["no_speech"] = torch.zeros(cap, dtype=torch.float32, device=dev)
         ses["full"] = torch.empty((cap, qk_rows, V), dtype=torch.float32, device=dev) if self.keep_full_logprobs else None
         ses["qk_buf"] = torch.zeros((cap, max(1, n_slots), qk_rows, N_CTX_AUDIO), dtype=torch.float32, device=dev)
-        # a batch's alignment rows are collected here (allocated once: no multi-GB allocation per batch); while an
-        # earlier batch's rows still occupy it (not yet aligned and freed), a batch gets a copy of its own
+        # the alignment rows of a batch (or of a collection of continuous batching) are collected here (allocated once:
+        # no multi-GB allocation per batch); while earlier rows still occupy it (not yet aligned and freed), the rows
+        # get a copy of their own
         ses["qk_out"] = torch.zeros_like(ses["qk_buf"])
         ses["qk_out_idx"] = None
         ses["s_tok"] = torch.zeros(cap, **i32)
@@ -642,50 +646,140 @@ class CudaEngine:
                                     cap, D, ses["xs"].data_ptr(), st), "wts_embed")
         self._decoder_rows(ses["st8"], ses["xs"], cap, ses["seq_ids"], ses["s_pos"], ses["s_qkr"], ses["qk_buf"],
                            active=ses["s_act"])
-        self._final_logits_static(ses["xs"], cap, ses["logits"], ses["st8"], active=ses["s_act"])
+        self._final_logits(ses["xs"], cap, ses["logits"], hs=ses["st8"]["hs_fin"], row_mask=ses["s_act"])
         self.launches += 1
+
+    # ------------------------------------------------------------------ the life of a decode slot
+    # Token state of slot b, as wts_step_inputs and wts_decode_select read it: tokens[b, :n_tokens[b]], of which the
+    # first n_prompt[b] are the prompt; done[b] = 0 running, 1 ended by <|endoftext|>, 2 stopped at the decoding limit;
+    # logprobs[b, r]: log-prob of the token chosen at row r.  A window is seeded into a slot (_seed, inside _admit),
+    # decoded, and collected into a WindowRecord with its alignment rows (_collect).
+    def _park(self, ses):
+        """Every slot parked (one token, done): the step and select kernels skip it until a window is seeded into it."""
+        ses["tokens"].zero_()
+        ses["n_tokens"].fill_(1)
+        ses["n_prompt"].fill_(1)
+        ses["done"].fill_(1)
+        ses["logprobs"].zero_()
+
+    def _slot_index(self, slots):
+        """Index of `slots` in the session's per-slot tensors: a slice (views, in-place copies) when they are 0..n-1,
+        else a device index."""
+        slots = list(slots)
+        if slots == list(range(len(slots))):
+            return slice(0, len(slots))
+        return torch.as_tensor(slots, dtype=torch.long, device=self.dev)
+
+    def _seed(self, ses, slots, prompts):
+        """`prompts` written into `slots`, which are set running; the other slots keep their state."""
+        sel = self._slot_index(slots)
+        th = np.zeros((len(prompts), ses["tokens"].shape[1]), dtype=np.int32)
+        for k, p in enumerate(prompts):
+            th[k, :len(p)] = p
+        nt = np.array([len(p) for p in prompts], dtype=np.int32)
+        for key, rows in (("tokens", th), ("n_tokens", nt), ("n_prompt", nt)):
+            rows = torch.from_numpy(rows)
+            ses[key][sel] = rows if isinstance(sel, slice) else rows.to(self.dev)    # a slice view takes host rows
+        ses["done"][sel] = 0
+        ses["logprobs"][sel] = 0.0
+
+    def _admit(self, ses, batch, setup):
+        """Windows into decode slots, batch = [(slot, job)]: encoder, cross-attention K/V, token state, prompt prefill
+        and the first sampled token; the windows' <|nospeech|> probabilities stay in ses["no_speech"].  Slots 0..n-1
+        are written in place.  Other slots get their cross K/V through a staging buffer, and their first token is
+        selected with every other slot parked (the select kernel works on slots 0..rows-1)."""
+        st8 = ses["st8"]
+        n = len(batch)
+        slots = [s for s, _ in batch]
+        sel = self._slot_index(slots)
+        direct = isinstance(sel, slice)
+        with self.phase("encoder"):
+            xa = self.encode([j for _, j in batch])
+        with self.phase("cross_kv"):
+            if direct:
+                self._cross_kv(xa, st8, n)
+            else:
+                tmp = self._alloc_cross_state(n)
+                self._cross_kv(xa, tmp, n)
+                for li in range(self.dims.n_text_layer):
+                    for name in ("ck", "cv", "ckal"):
+                        if st8[name][li] is not None:
+                            st8[name][li].index_copy_(0, sel, tmp[name][li])
+                del tmp
+        del xa
+        prompts = [list(j["prompt"]) for _, j in batch]
+        self._seed(ses, slots, prompts)
+        with self.phase("prefill"):
+            logits2, no_speech = self._prefill(ses, prompts, slots, setup.tokenizer, qk_last=True)
+            if direct:
+                self._select(ses, logits2, n)
+            else:
+                cap = ses["cap"]
+                ses["logits"].index_copy_(0, sel, logits2[:n])
+                saved = ses["done"].clone()
+                ses["done"].fill_(1)
+                ses["done"].index_fill_(0, sel, 0)
+                self._select(ses, ses["logits"], cap)
+                mask = torch.zeros(cap, dtype=torch.bool, device=self.dev)
+                mask[sel] = True
+                ses["done"].copy_(torch.where(mask, ses["done"], saved))
+                self.launches += 4
+            ses["no_speech"][sel] = no_speech
+
+    def _collect(self, ses, batch, setup):
+        """Records of the windows decoded in batch = [(slot, job)], in that order.  Their alignment rows are kept as
+        one buffer: the session's qk_out when no earlier rows occupy it, else a copy of their own."""
+        dev = self.dev
+        n = len(batch)
+        sel = self._slot_index([s for s, _ in batch])
+        tokens_h, n_tok_h, done_h, lp_h, ns_h = (ses[k][sel].cpu().numpy()
+                                                 for k in ("tokens", "n_tokens", "done", "logprobs", "no_speech"))
+        prompts = [list(j["prompt"]) for _, j in batch]
+        n_new = n_tok_h - np.array([len(p) for p in prompts])          # sampled tokens of each window
+        max_rows = int(n_new.max()) + 1
+        qk_buf, held = ses["qk_buf"], ses["qk_out_idx"]
+        if held is None or held >= len(self.qk_buffers) or self.qk_buffers[held] is None:
+            rows = ses["qk_out"][:n]
+            ses["qk_out_idx"] = len(self.qk_buffers)
+        else:
+            rows = torch.empty((n, qk_buf.shape[1], max_rows, N_CTX_AUDIO), dtype=torch.float32, device=dev)
+        rows[:, :, :max_rows] = qk_buf[sel, :, :max_rows]
+        first = self._keep_rows(rows)
+        full = ses["full"]
+        if full is not None:
+            full = full[sel, :max_rows].clone()
+            self.full_logprobs.append(full)
+        limit = [k for k in range(n) if int(done_h[k]) == 2]
+        last_full = {}
+        if limit:       # windows that ran into the decoding limit: the reference may need chunk_logprobs[-1][fallback]
+            lf = ses["last_full"][torch.as_tensor([batch[k][0] for k in limit], device=dev)].cpu()
+            last_full = {k: lf[i] for i, k in enumerate(limit)}
+        records = []
+        for k, (_, job) in enumerate(batch):
+            P, n_k = len(prompts[k]), int(n_new[k])
+            ended = int(done_h[k]) == 1
+            n_rows = n_k + 1 if ended else n_k
+            last_lp = None
+            if k in last_full:
+                last_lp = (lambda t, row=last_full[k]: float(row[t]))
+            elif full is not None:
+                last_lp = (lambda t, kk=k, rr=n_rows - 1, ff=full: float(ff[kk, rr, t].item()))
+            records.append(WindowRecord(seek=job["seek"], segment_size=job["segment_size"], prompt=prompts[k],
+                                        tokens=tokens_h[k, P:P + n_k].tolist(), logprobs=lp_h[k, :n_rows].copy(),
+                                        ended_by_eot=ended, no_speech_prob=float(ns_h[k]), qk_window=first + k,
+                                        temperature=0.0, language=setup.tokenizer.language, last_row_logprobs=last_lp))
+        return records
 
     @torch.no_grad()
     def _decode_batch(self, jobs, setup):
-        d, dev = self.dims, self.dev
-        tok = setup.tokenizer
         B = len(jobs)
-        n_ctx = d.n_text_ctx
-        sample_len = setup.sample_len
         ses = self._decoder_session(setup, B)
-        cap, qk_rows = ses["cap"], ses["qk_rows"]
-        assert B <= cap
-        st8 = ses["st8"]
-        with self.phase("encoder"):
-            xa = self.encode(jobs)
-        prompts = [list(j["prompt"]) for j in jobs]
-        P = [len(p) for p in prompts]
-        with self.phase("cross_kv"):
-            self._cross_kv(xa, st8, B)
-        del xa
-
-        # ---- token state of this batch (slots >= B are parked as "done")
-        tokens_h = np.zeros((cap, n_ctx + 1), dtype=np.int32)
-        for b, p in enumerate(prompts):
-            tokens_h[b, :len(p)] = p
-        ses["tokens"].copy_(torch.from_numpy(tokens_h), non_blocking=False)
-        nt = np.ones(cap, dtype=np.int32)
-        nt[:B] = P
-        ses["n_tokens"].copy_(torch.from_numpy(nt))
-        ses["n_prompt"].copy_(torch.from_numpy(nt))
-        dn = np.ones(cap, dtype=np.int32)
-        dn[:B] = 0
-        ses["done"].copy_(torch.from_numpy(dn))
-        ses["logprobs"].zero_()
+        assert B <= ses["cap"]
+        self._park(ses)                            # slots >= B stay parked
         self._set_masks(ses, setup)
-        qk_buf = ses["qk_buf"]
-
-        with self.phase("prefill"):
-            logits2, no_speech = self._prefill(ses, prompts, range(B), tok, qk_last=True)
-            self._select(ses, logits2, B)
-
-        # ---- decode steps
-        max_steps = sample_len - 1
+        batch = list(enumerate(jobs))
+        self._admit(ses, batch, setup)
+        max_steps = setup.sample_len - 1
         steps_done = 0
         done = ses["done"]
         n_active = B
@@ -698,50 +792,7 @@ class CudaEngine:
         if self.profile:
             self.batch_log = getattr(self, "batch_log", [])
             self.batch_log.append((B, steps_done, len(self._events) - 1))
-        # ---- collect
-        torch.cuda.synchronize(dev)
-        tokens_h = ses["tokens"][:B].cpu().numpy()
-        n_tok_h = ses["n_tokens"][:B].cpu().numpy()
-        done_h = ses["done"][:B].cpu().numpy()
-        lp_h = ses["logprobs"][:B].cpu().numpy()
-        ns_h = no_speech.cpu().numpy()
-        max_rows = int(max(1, (n_tok_h - np.asarray(P)).max() + 1))
-        buf_idx = len(self.qk_buffers)
-        i = ses["qk_out_idx"]                                         # the session buffer is reused by the next batch
-        if i is None or i >= len(self.qk_buffers) or self.qk_buffers[i] is None:
-            rows = ses["qk_out"][:B]
-            rows[:, :, :max_rows].copy_(qk_buf[:B, :, :max_rows])
-            ses["qk_out_idx"] = buf_idx
-        else:
-            rows = qk_buf[:B, :, :max_rows].clone()
-        self.qk_buffers.append(rows)
-        full = ses["full"]
-        if full is not None:
-            self.full_logprobs.append(full[:B, :max_rows].clone())
-            full = self.full_logprobs[-1]
-        limit_rows = [b for b in range(B) if int(done_h[b]) == 2]
-        last_full_h = {}
-        if limit_rows:      # windows that ran into the decoding limit: the reference may need chunk_logprobs[-1][fallback]
-            lf = ses["last_full"][torch.as_tensor(limit_rows, device=dev)].cpu()
-            last_full_h = {b: lf[i] for i, b in enumerate(limit_rows)}
-        records = []
-        for b, job in enumerate(jobs):
-            n = int(n_tok_h[b] - P[b])
-            ended = int(done_h[b]) == 1
-            rows = n + 1 if ended else n
-            sampled = tokens_h[b, P[b]:P[b] + n].tolist()
-            gid = len(self.window_index)
-            self.window_index.append((buf_idx, b))
-            last_lp = None
-            if b in last_full_h:
-                last_lp = (lambda t, row=last_full_h[b]: float(row[t]))
-            elif full is not None:
-                last_lp = (lambda t, bb=b, rr=rows - 1, ff=full: float(ff[bb, rr, t].item()))
-            records.append(WindowRecord(seek=job["seek"], segment_size=job["segment_size"], prompt=prompts[b],
-                                        tokens=sampled, logprobs=lp_h[b, :rows].copy(), ended_by_eot=ended,
-                                        no_speech_prob=float(ns_h[b]), qk_window=gid, temperature=0.0,
-                                        language=tok.language, last_row_logprobs=last_lp))
-        return records
+        return self._collect(ses, batch, setup)
 
     # ------------------------------------------------------------------ continuous batching
     @torch.no_grad()
@@ -753,120 +804,41 @@ class CudaEngine:
         slowest window (a stuck one runs to the 224-token limit) before the follow-up windows even start.
         Same kernels, same per-window arithmetic as `decode_windows`; only the grouping of windows into steps differs.
         `collected()`, when given, is called after the records of each collection have been fed."""
-        d, dev = self.dims, self.dev
-        tok = setup.tokenizer
         assert not self.keep_full_logprobs, "decode_stream keeps no per-row log-prob tables"
-        n_ctx = d.n_text_ctx
         queue = list(jobs)
         if not queue:
             return
         ses = self._decoder_session(setup, min(self.batch_limit(setup), len(queue)))
-        cap, st8, qk_buf = ses["cap"], ses["st8"], ses["qk_buf"]
-        ses["done"].fill_(1)
+        cap = ses["cap"]
+        self._park(ses)
         self._set_masks(ses, setup)
         slot_job = [None] * cap               # job decoded in each slot
-        slot_info = [None] * cap              # (prompt, no_speech_prob)
         free = list(range(cap))
         max_steps = setup.sample_len - 1
-
-        def admit(batch):
-            """batch: list of (slot, job).  Encoder + cross K/V + prompt prefill + first token of the new windows."""
-            n = len(batch)
-            slots = [b for b, _ in batch]
-            d_slots = torch.as_tensor(slots, dtype=torch.long, device=dev)
-            with self.phase("encoder"):
-                xa = self.encode([j for _, j in batch])
-            with self.phase("cross_kv"):
-                if slots == list(range(n)):            # first admission: the windows land in slots 0 .. n-1 directly
-                    self._cross_kv(xa, st8, n)
-                else:
-                    tmp = self._alloc_cross_state(n)
-                    self._cross_kv(xa, tmp, n)
-                    for li in range(d.n_text_layer):
-                        for name in ("ck", "cv", "ckal"):
-                            if st8[name][li] is not None:
-                                st8[name][li].index_copy_(0, d_slots, tmp[name][li])
-                    del tmp
-                del xa
-            prompts = [list(j["prompt"]) for _, j in batch]
-            P = [len(p) for p in prompts]
-            th = np.zeros((n, n_ctx + 1), dtype=np.int32)
-            for k, p in enumerate(prompts):
-                th[k, :len(p)] = p
-            ses["tokens"].index_copy_(0, d_slots, torch.from_numpy(th).to(dev))
-            nt = torch.as_tensor(P, dtype=torch.int32, device=dev)
-            ses["n_tokens"].index_copy_(0, d_slots, nt)
-            ses["n_prompt"].index_copy_(0, d_slots, nt)
-            ses["logprobs"].index_fill_(0, d_slots, 0.0)
-            with self.phase("prefill"):
-                logits2, no_speech = self._prefill(ses, prompts, slots, tok, qk_last=True)
-                # first token of the new windows only: the select kernel works slot-wise, so the other slots are parked
-                ses["logits"].index_copy_(0, d_slots, logits2[:n])
-                saved = ses["done"].clone()
-                ses["done"].fill_(1)
-                ses["done"].index_fill_(0, d_slots, 0)
-                self._select(ses, ses["logits"], cap)
-                mask = torch.zeros(cap, dtype=torch.bool, device=dev)
-                mask[d_slots] = True
-                ses["done"].copy_(torch.where(mask, ses["done"], saved))
-                self.launches += 4
-            ns = no_speech.cpu().numpy()
-            for k, (b, job) in enumerate(batch):
-                slot_job[b] = job
-                slot_info[b] = (prompts[k], float(ns[k]))
-
-        def collect(finished, done_h):
-            """Records of the finished slots (their alignment rows are copied out: the slot is about to be reused)."""
-            d_f = torch.as_tensor(finished, dtype=torch.long, device=dev)
-            tokens_h = ses["tokens"].index_select(0, d_f).cpu().numpy()
-            n_tok_h = ses["n_tokens"].index_select(0, d_f).cpu().numpy()
-            lp_h = ses["logprobs"].index_select(0, d_f).cpu().numpy()
-            limit = [k for k, b in enumerate(finished) if int(done_h[b]) == 2]
-            last_rows = {}
-            if limit:
-                lf = ses["last_full"].index_select(0, d_f[torch.as_tensor(limit, device=dev)]).cpu()
-                last_rows = {k: lf[i] for i, k in enumerate(limit)}
-            out = []
-            n_rows = [int(n_tok_h[k]) - len(slot_info[b][0]) + (1 if int(done_h[b]) == 1 else 0) for k, b in enumerate(finished)]
-            buf_idx = len(self.qk_buffers)                   # one alignment buffer per collection (rows up to its longest window)
-            self.qk_buffers.append(qk_buf.index_select(0, d_f)[:, :, :max(1, max(n_rows))].contiguous())
-            for k, b in enumerate(finished):
-                prompt, ns = slot_info[b]
-                job = slot_job[b]
-                n = int(n_tok_h[k]) - len(prompt)
-                ended = int(done_h[b]) == 1
-                rows = n + 1 if ended else n
-                gid = len(self.window_index)
-                self.window_index.append((buf_idx, k))
-                last_lp = (lambda t, row=last_rows[k]: float(row[t])) if k in last_rows else None
-                out.append((job, WindowRecord(seek=job["seek"], segment_size=job["segment_size"], prompt=prompt,
-                                              tokens=tokens_h[k, len(prompt):len(prompt) + n].tolist(), logprobs=lp_h[k, :rows].copy(),
-                                              ended_by_eot=ended, no_speech_prob=ns, qk_window=gid, temperature=0.0,
-                                              language=tok.language, last_row_logprobs=last_lp)))
-                slot_job[b] = slot_info[b] = None
-            return out
-
         done = ses["done"]
         while queue or any(j is not None for j in slot_job):
             if queue and free:
                 batch = []
                 while queue and free:
                     batch.append((free.pop(0), queue.pop(0)))
-                admit(batch)
+                self._admit(ses, batch, setup)
+                for b, job in batch:
+                    slot_job[b] = job
             with self.phase("decode_steps"):
                 n_active = int((done == 0).sum().item())
                 if n_active > 0:
                     self._decode_chunk(ses, n_active, 8, max_steps)
             done_h = done.cpu().numpy()
-            finished = [b for b in range(cap) if slot_job[b] is not None and int(done_h[b]) != 0]
+            finished = [(b, slot_job[b]) for b in range(cap) if slot_job[b] is not None and int(done_h[b]) != 0]
             if finished:
-                for job, rec in collect(finished, done_h):
+                for (b, job), rec in zip(finished, self._collect(ses, finished, setup)):
+                    slot_job[b] = None
                     nxt = feed(job, rec)
                     if nxt is not None:
                         queue.append(nxt)
                 if collected is not None:
                     collected()
-                free.extend(finished)
+                free.extend(b for b, _ in finished)
                 free.sort()
 
     # ------------------------------------------------------------------ beam search / sampling (upstream strategies)
@@ -902,16 +874,8 @@ class CudaEngine:
         del xa
         prompt = list(job["prompt"])
         P = len(prompt)
-        tokens_h = np.zeros((cap, n_ctx + 1), dtype=np.int32)
-        tokens_h[:G, :P] = prompt
-        ses["tokens"].copy_(torch.from_numpy(tokens_h))
-        nt = np.ones(cap, dtype=np.int32)
-        nt[:G] = P
-        ses["n_tokens"].copy_(torch.from_numpy(nt))
-        ses["n_prompt"].copy_(torch.from_numpy(nt))
-        dn = np.ones(cap, dtype=np.int32)
-        dn[:G] = 0
-        ses["done"].copy_(torch.from_numpy(dn))
+        self._park(ses)
+        self._seed(ses, range(G), [prompt] * G)
         self._set_masks(ses, setup)
         # ---- prefill of hypothesis 0, then its self-attention cache is shared out
         with self.phase("prefill"):
@@ -929,68 +893,68 @@ class CudaEngine:
         sum_lp = torch.zeros(G, dtype=torch.float32)              # float32 arithmetic like upstream's tensor
         finished = {}                                              # beam search: sequence (tuple) -> cumulative log-prob
         max_candidates = round(beam * (setup.patience or 1.0)) if beam else 0
-        ph = self.phase("decode_steps")
-        ph.__enter__()
-        for i in range(setup.sample_len):
-            nat.check(nat.lib.wts_filtered_logprobs(ses["logits"].data_ptr(), V, ctypes.byref(ses["cfg"]), ses["suppress"].data_ptr(),
-                                                    ses["blank"].data_ptr(), ses["tokens"].data_ptr(), ses["n_tokens"].data_ptr(),
-                                                    ses["n_prompt"].data_ptr(), lp_dev.data_ptr(), G, st), "wts_filtered_logprobs")
-            self.launches += 1
-            source = list(range(G))
-            if beam:
-                vals, idxs = torch.topk(lp_dev[:G], beam + 1, dim=-1)
-                vals, idxs = vals.cpu(), idxs.cpu()
-                scores, sources = {}, {}
-                for j in range(G):
-                    prefix = seqs[j]
-                    for logprob, token in zip(vals[j], idxs[j]):
-                        sequence = tuple(prefix + [int(token)])
-                        scores[sequence] = (sum_lp[j] + logprob).item()
-                        sources[sequence] = j
-                new_seqs, source, newly_finished = [], [], {}
-                for sequence in sorted(scores, key=scores.get, reverse=True):
-                    if sequence[-1] == tok.eot:
-                        newly_finished[sequence] = scores[sequence]
-                    else:
-                        sum_lp[len(new_seqs)] = scores[sequence]
-                        new_seqs.append(list(sequence))
-                        source.append(sources[sequence])
-                        if len(new_seqs) == beam:
+        with self.phase("decode_steps"):
+            for i in range(setup.sample_len):
+                nat.check(nat.lib.wts_filtered_logprobs(ses["logits"].data_ptr(), V, ctypes.byref(ses["cfg"]),
+                                                        ses["suppress"].data_ptr(), ses["blank"].data_ptr(),
+                                                        ses["tokens"].data_ptr(), ses["n_tokens"].data_ptr(),
+                                                        ses["n_prompt"].data_ptr(), lp_dev.data_ptr(), G, st),
+                          "wts_filtered_logprobs")
+                self.launches += 1
+                source = list(range(G))
+                if beam:
+                    vals, idxs = torch.topk(lp_dev[:G], beam + 1, dim=-1)
+                    vals, idxs = vals.cpu(), idxs.cpu()
+                    scores, sources = {}, {}
+                    for j in range(G):
+                        prefix = seqs[j]
+                        for logprob, token in zip(vals[j], idxs[j]):
+                            sequence = tuple(prefix + [int(token)])
+                            scores[sequence] = (sum_lp[j] + logprob).item()
+                            sources[sequence] = j
+                    new_seqs, source, newly_finished = [], [], {}
+                    for sequence in sorted(scores, key=scores.get, reverse=True):
+                        if sequence[-1] == tok.eot:
+                            newly_finished[sequence] = scores[sequence]
+                        else:
+                            sum_lp[len(new_seqs)] = scores[sequence]
+                            new_seqs.append(list(sequence))
+                            source.append(sources[sequence])
+                            if len(new_seqs) == beam:
+                                break
+                    for seq in sorted(newly_finished, key=newly_finished.get, reverse=True):
+                        if len(finished) >= max_candidates:
                             break
-                for seq in sorted(newly_finished, key=newly_finished.get, reverse=True):
-                    if len(finished) >= max_candidates:
-                        break
-                    finished[seq] = newly_finished[seq]
-                seqs = new_seqs
-                completed = len(finished) >= max_candidates
-            else:
-                lp = lp_dev[:G].cpu()
-                nxt = torch.distributions.Categorical(logits=lp / T).sample()
-                last = torch.tensor([s_[-1] for s_ in seqs])
-                sum_lp += lp[torch.arange(G), nxt] * (last != tok.eot)
-                nxt[last == tok.eot] = tok.eot
-                for s_, t_ in zip(seqs, nxt.tolist()):
-                    s_.append(t_)
-                completed = bool((nxt == tok.eot).all())
-            cur = len(seqs[0])
-            if completed or cur > n_ctx:
-                break
-            if i + 1 == setup.sample_len:
-                break
-            # ---- device state follows the host: caches of the source hypotheses, new token rows, next logits
-            if source != list(range(G)):
-                src = torch.as_tensor(source, dtype=torch.long, device=dev)
-                for li in range(L):
-                    for name in ("sk", "sv"):
-                        t = st8[name][li]
-                        t[:G, :, :cur - 1] = t[src, :, :cur - 1]
-            th = np.zeros((G, n_ctx + 1), dtype=np.int32)
-            for r, s_ in enumerate(seqs):
-                th[r, :cur] = s_
-            ses["tokens"][:G].copy_(torch.from_numpy(th))
-            ses["n_tokens"][:G].fill_(cur)
-            self._step_logits(ses)
-        ph.__exit__()
+                        finished[seq] = newly_finished[seq]
+                    seqs = new_seqs
+                    completed = len(finished) >= max_candidates
+                else:
+                    lp = lp_dev[:G].cpu()
+                    nxt = torch.distributions.Categorical(logits=lp / T).sample()
+                    last = torch.tensor([s_[-1] for s_ in seqs])
+                    sum_lp += lp[torch.arange(G), nxt] * (last != tok.eot)
+                    nxt[last == tok.eot] = tok.eot
+                    for s_, t_ in zip(seqs, nxt.tolist()):
+                        s_.append(t_)
+                    completed = bool((nxt == tok.eot).all())
+                cur = len(seqs[0])
+                if completed or cur > n_ctx:
+                    break
+                if i + 1 == setup.sample_len:
+                    break
+                # ---- device state follows the host: caches of the source hypotheses, new token rows, next logits
+                if source != list(range(G)):
+                    src = torch.as_tensor(source, dtype=torch.long, device=dev)
+                    for li in range(L):
+                        for name in ("sk", "sv"):
+                            t = st8[name][li]
+                            t[:G, :, :cur - 1] = t[src, :, :cur - 1]
+                th = np.zeros((G, n_ctx + 1), dtype=np.int32)
+                for r, s_ in enumerate(seqs):
+                    th[r, :cur] = s_
+                ses["tokens"][:G].copy_(torch.from_numpy(th))
+                ses["n_tokens"][:G].fill_(cur)
+                self._step_logits(ses)
         # ---- finalize + rank (upstream BeamSearchDecoder.finalize / GreedyDecoder.finalize, MaximumLikelihoodRanker)
         if beam:
             if len(finished) < beam:
@@ -1017,12 +981,6 @@ class CudaEngine:
         return WindowRecord(seek=job["seek"], segment_size=job["segment_size"], prompt=prompt, tokens=cut[best], logprobs=None,
                             ended_by_eot=True, no_speech_prob=float(no_speech.cpu()[0]), qk_window=-1, temperature=T,
                             language=tok.language, sum_logprob=float(cand_lp[best]))
-
-    def _final_logits_static(self, x_rows, n_rows, logits, st8, active=None):
-        d, w = self.dims, self.w
-        hs = st8["hs_fin"]
-        self.layernorm(x_rows, w.ln_g, w.ln_b, n_rows, d.n_text_state, out_sb=hs)
-        self.gemm(hs, w.emb_sb, n_rows, d.n_vocab, d.n_text_state, out_f32=logits, ldc=d.n_vocab, row_mask=active)
 
     # ------------------------------------------------------------------ teacher-forced pass (two-pass strategy)
     @torch.no_grad()
@@ -1073,11 +1031,7 @@ class CudaEngine:
                                                      out.data_ptr(), len(pairs), st), "wts_logprob_gather")
                 self.launches += 2
                 vals = out.cpu().numpy()
-        buf_idx = len(self.qk_buffers)
-        self.qk_buffers.append(qk_buf)
-        gid = len(self.window_index)
-        self.window_index.append((buf_idx, 0))
-        return gid, vals
+        return self._keep_rows(qk_buf), vals
 
     # ------------------------------------------------------------------ language detection
     @torch.no_grad()
@@ -1139,6 +1093,15 @@ class CudaEngine:
                 for (i, _, _), l_ in zip(lst, split_jumps(dl.cpu().numpy(), plan)):
                     lefts[i] = l_[:-1]
         return (out, lefts) if disfluencies else out
+
+    def _keep_rows(self, rows):
+        """Keeps the alignment rows [windows, heads, rows, 1500] of a decode batch, a collection or a teacher-forced
+        segment as one buffer for align(); returns the window id of its first window (the others follow in order)."""
+        buf, first = len(self.qk_buffers), len(self.window_index)
+        self.qk_buffers.append(rows)
+        for b in range(rows.shape[0]):
+            self.window_index.append((buf, b))
+        return first
 
     def free_alignment_rows(self, windows):
         """Drop the alignment rows of the decode batches holding these (already aligned) windows."""
