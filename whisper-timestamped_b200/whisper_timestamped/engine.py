@@ -767,7 +767,8 @@ class CudaEngine:
             records.append(WindowRecord(seek=job["seek"], segment_size=job["segment_size"], prompt=prompts[k],
                                         tokens=tokens_h[k, P:P + n_k].tolist(), logprobs=lp_h[k, :n_rows].copy(),
                                         ended_by_eot=ended, no_speech_prob=float(ns_h[k]), qk_window=first + k,
-                                        temperature=0.0, language=setup.tokenizer.language, last_row_logprobs=last_lp))
+                                        temperature=0.0, language=job.get("language", setup.tokenizer.language),
+                                        last_row_logprobs=last_lp))
         return records
 
     @torch.no_grad()
@@ -1034,30 +1035,44 @@ class CudaEngine:
         return self._keep_rows(qk_buf), vals
 
     # ------------------------------------------------------------------ language detection
-    @torch.no_grad()
     def detect_language(self, mel, tokenizer):
         """Upstream detect_language on the first 30 s: logits at <|startoftranscript|>, softmax over the
         language tokens (T.py:862-867 exposes the same numbers as language_probs)."""
+        return self.detect_languages([mel], tokenizer)[0]
+
+    @torch.no_grad()
+    def detect_languages(self, mels, tokenizer):
+        """detect_language for many recordings: one encoder pass over their first windows (in batches of at most
+        `max_batch`, fewer when that many windows would not fit in 85 % of the free device memory, as batch_limit
+        sizes a decode batch), then one decoder row per recording at <|startoftranscript|>.  Returns [(language, probs)]."""
         d, dev, st, w = self.dims, self.dev, self._st(), self.w
-        size = min(N_FRAMES, int(mel.shape[0]))
-        job = dict(mel=mel, seek=0, segment_size=size)
-        xa = self.encode([job])
-        st8 = self._alloc_decoder_state(1, 1)
-        self._cross_kv(xa, st8, 1)
-        qk_buf = torch.zeros((1, len(self.heads), 1, N_CTX_AUDIO), dtype=torch.float32, device=dev)
-        x = torch.empty((1, d.n_text_state), dtype=torch.float32, device=dev)
-        one = _i32([0], dev)
-        t = _i32([tokenizer.sot], dev)
-        nat.check(nat.lib.wts_embed(t.data_ptr(), one.data_ptr(), w.emb.data_ptr(), w.dec_pos.data_ptr(), 1, d.n_text_state,
-                                    x.data_ptr(), st), "wts_embed")
-        self._decoder_rows(st8, x, 1, one, one, _i32([-1], dev), qk_buf)
-        logits = torch.empty((1, d.n_vocab), dtype=torch.float32, device=dev)
-        self._final_logits(x, 1, logits)
-        lg = logits[0].cpu()
         ids = list(tokenizer.all_language_tokens)
-        probs = torch.softmax(lg[ids].float(), dim=-1).tolist()
-        language_probs = dict(zip(tokenizer.all_language_codes, probs))
-        return max(language_probs, key=language_probs.get), language_probs
+        torch.cuda.empty_cache()
+        free, _ = torch.cuda.mem_get_info(dev)
+        step = max(1, min(self.max_batch, int(0.85 * free) // self.window_bytes(1)))
+        out = []
+        for i in range(0, len(mels), step):
+            part = mels[i:i + step]
+            B = len(part)
+            xa = self.encode([dict(mel=m, seek=0, segment_size=min(N_FRAMES, int(m.shape[0]))) for m in part])
+            st8 = self._alloc_decoder_state(B, B)
+            self._cross_kv(xa, st8, B)
+            del xa
+            qk_buf = torch.zeros((B, len(self.heads), 1, N_CTX_AUDIO), dtype=torch.float32, device=dev)
+            x = torch.empty((B, d.n_text_state), dtype=torch.float32, device=dev)
+            seq, pos = _i32(list(range(B)), dev), _i32([0] * B, dev)
+            t = _i32([tokenizer.sot] * B, dev)
+            nat.check(nat.lib.wts_embed(t.data_ptr(), pos.data_ptr(), w.emb.data_ptr(), w.dec_pos.data_ptr(), B,
+                                        d.n_text_state, x.data_ptr(), st), "wts_embed")
+            self._decoder_rows(st8, x, B, seq, pos, _i32([-1] * B, dev), qk_buf)
+            logits = torch.empty((B, d.n_vocab), dtype=torch.float32, device=dev)
+            self._final_logits(x, B, logits)
+            self.launches += 1
+            del st8
+            for row in torch.softmax(logits[:, ids].cpu().float(), dim=-1).tolist():
+                probs = dict(zip(tokenizer.all_language_codes, row))
+                out.append((max(probs, key=probs.get), probs))
+        return out
 
     # ------------------------------------------------------------------ alignment
     def align(self, items, disfluencies=False):

@@ -1,8 +1,9 @@
 """Host-only helpers the reference's command line uses to write a result dict to text formats
 (/root/reference/whisper_timestamped/transcribe.py:2298-2323 `flatten`, `remove_keys`, `write_csv`; 3183-3199
-`filtered_keys`).  The CSV / TSV layouts are pinned by the reference's fixtures tests/expected/punctuations_* (replayed
-by tests/test_subtitles.py).  The txt / srt / vtt writers of the reference's CLI come from openai-whisper and are not
-restated here; `make_subtitles.py` holds the reference's own srt / vtt writers.
+`filtered_keys`), and the txt / srt / vtt writers it takes from openai-whisper (`get_writer(fmt).write_result` with
+`highlight_words=False` and no line width or count, T.py:2982-2999).  Every layout is pinned byte for byte by the files
+the reference's command line wrote, tests/expected/punctuations_* (replayed by tests/test_subtitles.py and
+tests/test_cli_writers.py).
 """
 import csv
 
@@ -49,3 +50,23 @@ def filtered_keys(result, keys=KEPT_KEYS):
     if isinstance(result, float):
         return round(result, 2)
     return result
+
+
+def write_txt(transcript, file):
+    """One line per segment: its stripped text."""
+    for segment in transcript:
+        print(segment["text"].strip(), file=file, flush=True)
+
+
+def write_srt(transcript, file):
+    """SubRip cues numbered from 1, `hh:mm:ss,mmm` times, `-->` in the text written `->`."""
+    from .make_subtitles import write_srt as cues
+    cues(list(transcript), file=file)
+
+
+def write_vtt(transcript, file):
+    """WebVTT cues, `[hh:]mm:ss.mmm` times.  The `.vtt` and `.words.vtt` files of the reference's command line start
+    with the `WEBVTT` header twice; the same bytes are written here."""
+    from .make_subtitles import write_vtt as cues
+    print("WEBVTT\n", file=file)
+    cues(list(transcript), file=file)
