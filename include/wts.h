@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define WTS_VERSION 102
+#define WTS_VERSION 103
 #define WTS_SEG_NONPOSITIVE 1
 #define WTS_SEG_PITCH16 2
 
@@ -151,6 +151,8 @@ typedef struct WtsGemm {
     int32_t a_is_f32, b_is_f32;   /* SIMT backend only: operand is plain float32 (log-mel DFT / filterbank GEMMs) */
     const int32_t* row_mask;  /* optional [M] (M <= 128, unbatched): rows with mask 0 are skipped, their outputs stay
                                  untouched (finished windows of a decode batch); NULL = every row */
+    int32_t b_const;          /* 1: B is a model weight that no kernel still in flight on the stream writes, so a
+                                 decode-time GEMM may start loading B before the previous kernel has completed */
 } WtsGemm;
 
 /* Error-compensated GEMM.  Replaces every torch Linear / Conv1d / matmul of the encoder and decoder. */

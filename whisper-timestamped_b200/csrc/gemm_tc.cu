@@ -5,11 +5,11 @@
 // (the dropped lo*lo term is ~2^-16 relative).  That keeps logits and cross-attention scores within
 // the 1e-3 bar of the reference's float32 CPU path while running on the tensor cores.
 //
-// Both kernels feed 128 x 128 output tiles from the same operand ring: per k-block the TMA producer lane loads 4 boxes
+// The first two kernels feed 128 x 128 output tiles from the same operand ring: per k-block the TMA producer lane loads 4 boxes
 // (A_hi, A_lo, B_hi, B_lo; 128 rows x 64 bf16, SWIZZLE_128B) into one of 3 stages; full[s] completes on the byte
 // count, empty[s] once the consumer warps have retired the k-block's wgmmas.  Batched problems (two batch levels) are
 // extra tensor-map dimensions; M/N/K tails rely on TMA zero fill.  Every output element sums the same k-blocks, k16
-// steps and terms (hi*hi, lo*hi, hi*lo) in the same order in both kernels, so they give bit-identical results.
+// steps and terms (hi*hi, lo*hi, hi*lo) in the same order in every kernel here, so they give bit-identical results.
 //
 // gemm_tc_kernel (encoder, cross-K/V, prefill: more than one M tile, batched, or head-major output): persistent,
 // warp-specialized, ping-pong.  grid = min(tiles, SMs), 384 threads:
@@ -27,6 +27,14 @@
 // in its own shared memory (the idle operand ring), the cluster synchronises, and CTA r reduces rows r, r + S, ... of
 // all S partials over distributed shared memory (ld.shared::cluster) and applies the epilogue to them: no atomics, no
 // global workspace, a fixed summation order (bit-reproducible), and the epilogue itself is spread over S SMs.
+//
+// gemm_tc_skinny64_kernel (the same with M <= 64: a decode step of a session of at most 64 windows).  One 64-row A box
+// (no wgmma on zero-filled rows), one consumer warpgroup plus the TMA warp (160 threads), a 4-stage ring of 48 KB stages.
+// A CTA streams only 2..10 k-blocks (20 for the vocabulary projection), so its time is round trips to HBM, not bytes.
+// With WtsGemm::b_const the producer issues the weight (B) boxes of all four ring stages before the dependency wait:
+// the whole share of a D x D GEMM's CTA and most of a QKV / FC1 CTA's are in flight while the previous kernel runs.
+// Split, k-block partition, wgmma sequence, partial-sum order and epilogue are those of gemm_tc_skinny_kernel: its rows
+// are bit-identical to the rows 0..63 of the 128-row kernel.
 #include <cuda_bf16.h>
 
 #include <stdlib.h>
@@ -47,6 +55,14 @@ constexpr int GROUP_M = 8;                              // M tiles per raster gr
 constexpr int GT_SMEM = STAGES * STAGE_BYTES + 256 + 1024;
 constexpr int PART_LD = BN + 4;                         // float pitch of a parked partial tile
 static_assert(BM * PART_LD * 4 <= STAGES * STAGE_BYTES, "the partial tile lives in the operand ring");
+constexpr int SK_BM = 64;                               // one-tile variant: rows of its A box
+constexpr int SK_A_BYTES = SK_BM * BK * 2;              // 8 KB
+constexpr int SK_STAGES = 4;                            // measured: 2 and 3 stages are slower
+constexpr int SK_STAGE_BYTES = 2 * SK_A_BYTES + 2 * TILE_BYTES;   // A_hi, A_lo, B_hi, B_lo: 48 KB
+constexpr int SK_THREADS = 160;                         // one consumer warpgroup + the TMA warp
+constexpr int SK_SMEM = SK_STAGES * SK_STAGE_BYTES + 256 + 1024;
+static_assert(SK_BM * PART_LD * 4 <= SK_STAGES * SK_STAGE_BYTES, "the partial tile lives in the operand ring");
+static_assert(SK_SMEM <= 227 * 1024, "the 64-row kernel's ring fits in an SM's shared memory");
 
 __device__ __forceinline__ float gelu_erf_tc(float v) { return 0.5f * v * (1.0f + erff(v * 0.70710678118654752440f)); }
 
@@ -156,6 +172,19 @@ __device__ __forceinline__ void epilogue_frag64(const WtsGemm& g, int zo, int zi
             }
         }
     }
+}
+
+// element (m, n) of a K-split tile: the S <= 8 partials x[0..S) summed in rank order (the zeros past S add nothing),
+// then the epilogue
+__device__ __forceinline__ void split_epilogue_one(const WtsGemm& g, int m, int n, const float (&x)[8], float bias_n)
+{
+    float t = 0.f;
+#pragma unroll
+    for (int s = 0; s < 8; ++s) t += x[s];
+    t = g.alpha * t + (g.bias ? (g.bias_on_m ? g.bias[m] : bias_n) : 0.f);
+    if (g.act == 1) t = gelu_erf_tc(t);
+    if (g.residual) t += g.residual[(int64_t)m * g.ldr + n];
+    store_one(g, m, n, t, g.out_f32, reinterpret_cast<__nv_bfloat16*>(g.out_sb16));
 }
 
 __device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
@@ -384,8 +413,6 @@ gemm_tc_skinny_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
                     if (s < S) asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(peer[s]) : "r"(base + 4u * c), "r"(s));
                 }
                 const float bias_n = (g.bias && !g.bias_on_m) ? g.bias[n] : 0.f;
-                float* of = g.out_f32;
-                __nv_bfloat16* ob = reinterpret_cast<__nv_bfloat16*>(g.out_sb16);
 #pragma unroll 1
                 for (int m = (int)rank + S * half; m < g.M; m += 2 * S) {
                     if (g.row_mask && g.row_mask[m] == 0) continue;
@@ -395,13 +422,145 @@ gemm_tc_skinny_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
                         x[s] = 0.f;
                         if (s < S) asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(x[s]) : "r"(peer[s] + (uint32_t)(m * PART_LD * 4)));
                     }
-                    float t = 0.f;
+                    split_epilogue_one(g, m, n, x, bias_n);
+                }
+            }
+        }
+        __syncwarp();
+        cluster_sync_all();                          // nobody leaves while a peer may still read its partial tile
+    }
+}
+
+__global__ void __launch_bounds__(SK_THREADS, 1)
+gemm_tc_skinny64_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcArgs args)
+{
+    extern __shared__ unsigned char smem_raw[];
+    const WtsGemm& g = args.g;
+    const uint32_t base = (smem_addr(smem_raw) + 1023u) & ~1023u;
+    const uint32_t bar = base + SK_STAGES * SK_STAGE_BYTES;   // full[s] at +8s, empty[s] at +32+8s
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int n0 = blockIdx.x * BN;
+    const int S = args.split_k;
+    const int nkb_all = (g.K + BK - 1) / BK;
+    const int kb0 = (int)((int64_t)blockIdx.z * nkb_all / S);
+    const int nkb = (int)((int64_t)(blockIdx.z + 1) * nkb_all / S) - kb0;
+    pdl_launch();
+
+    if (threadIdx.x == 128) {
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
+        for (int s = 0; s < SK_STAGES; ++s) { mbar_init(bar + 8 * s, 1); mbar_init(bar + 32 + 8 * s, 4); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    float acc[64];
+    if (warp == 4) {
+        if (lane == 0) {
+            // the weights are not written by any earlier kernel of the stream: the first stages' B boxes are issued
+            // before the dependency wait, their A (activation) boxes after it, on the same full barriers
+            const int pre = g.b_const ? min(nkb, SK_STAGES) : 0;
+            for (int kb = 0; kb < pre; ++kb) {
+                const uint32_t st = base + kb * SK_STAGE_BYTES, full = bar + 8 * kb;
+                mbar_expect_tx(full, SK_STAGE_BYTES);
+                tma_load_5d(st + 2 * SK_A_BYTES, &tmB, full, (kb0 + kb) * BK, n0, 0, 0, 0);
+                tma_load_5d(st + 2 * SK_A_BYTES + TILE_BYTES, &tmB, full, (kb0 + kb) * BK, n0, 0, 0, 1);
+            }
+            pdl_wait();
+            for (int kb = 0; kb < pre; ++kb) {
+                const uint32_t st = base + kb * SK_STAGE_BYTES, full = bar + 8 * kb;
+                tma_load_5d(st, &tmA, full, (kb0 + kb) * BK, 0, 0, 0, 0);
+                tma_load_5d(st + SK_A_BYTES, &tmA, full, (kb0 + kb) * BK, 0, 0, 0, 1);
+            }
+            for (int kb = pre; kb < nkb; ++kb) {
+                const int s = kb % SK_STAGES, u = kb / SK_STAGES;
+                mbar_wait(bar + 32 + 8 * s, (u & 1) ^ 1);
+                const uint32_t full = bar + 8 * s;
+                mbar_expect_tx(full, SK_STAGE_BYTES);
+                const uint32_t st = base + s * SK_STAGE_BYTES;
+                const int kc = (kb0 + kb) * BK;
+                tma_load_5d(st, &tmA, full, kc, 0, 0, 0, 0);
+                tma_load_5d(st + SK_A_BYTES, &tmA, full, kc, 0, 0, 0, 1);
+                tma_load_5d(st + 2 * SK_A_BYTES, &tmB, full, kc, n0, 0, 0, 0);
+                tma_load_5d(st + 2 * SK_A_BYTES + TILE_BYTES, &tmB, full, kc, n0, 0, 0, 1);
+            }
+        } else {
+            pdl_wait();
+        }
+    } else {
+        pdl_wait();                                 // the epilogue reads bias / residual / row mask written upstream
 #pragma unroll
-                    for (int s = 0; s < 8; ++s) t += x[s];                 // fixed order; the zeros past S add nothing
-                    t = g.alpha * t + (g.bias ? (g.bias_on_m ? g.bias[m] : bias_n) : 0.f);
-                    if (g.act == 1) t = gelu_erf_tc(t);
-                    if (g.residual) t += g.residual[(int64_t)m * g.ldr + n];
-                    store_one(g, m, n, t, of, ob);
+        for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+        for (int kb = 0; kb < nkb; ++kb) {
+            const int s = kb % SK_STAGES, u = kb / SK_STAGES;
+            mbar_wait(bar + 8 * s, u & 1);
+            const uint32_t st = base + s * SK_STAGE_BYTES;
+            const uint64_t a_hi = wg_desc(st), a_lo = wg_desc(st + SK_A_BYTES);
+            const uint64_t b_hi = wg_desc(st + 2 * SK_A_BYTES), b_lo = wg_desc(st + 2 * SK_A_BYTES + TILE_BYTES);
+            wg_fence();
+#pragma unroll
+            for (int k = 0; k < BK / 16; ++k) {
+                const uint64_t adv = (uint64_t)(k * 2);       // 32 bytes per K=16 step, in 16-byte units
+                wgmma_ss_n128(acc, a_hi + adv, b_hi + adv, 1);
+                wgmma_ss_n128(acc, a_lo + adv, b_hi + adv, 1);
+                wgmma_ss_n128(acc, a_hi + adv, b_lo + adv, 1);
+            }
+            wg_commit();
+            wg_wait<1>();                                     // the previous k-block's wgmmas have retired
+            if (kb > 0 && lane == 0) mbar_arrive(bar + 32 + 8 * ((kb - 1) % SK_STAGES));
+        }
+        wg_wait<0>();
+
+        if (S == 1) {
+            epilogue_frag64<false>(g, 0, 0, 16 * warp, n0, acc);
+        } else {
+            // every TMA write has landed (all full barriers were waited) and every wgmma has retired: the ring is idle
+            asm volatile("bar.sync 1, 128;" ::: "memory");
+            float* part = reinterpret_cast<float*>(smem_raw + (base - smem_addr(smem_raw)));
+            const int rl = 16 * warp + (lane >> 2), cl = 2 * (lane & 3);
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+#pragma unroll
+                for (int j = 0; j < 16; ++j)
+                    *reinterpret_cast<float2*>(part + (rl + 8 * i) * PART_LD + cl + 8 * j) =
+                        make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+        }
+    }
+    if (S > 1) {
+        __syncwarp();
+        cluster_sync_all();                          // every partial tile is parked and visible cluster-wide
+        if (threadIdx.x < 128) {
+            // CTA r reduces rows r + S * (4i + warp); a lane owns 4 adjacent columns and reads them from each of
+            // the S partial tiles with one 16-byte distributed-shared-memory load
+            uint32_t rank;
+            asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(rank));
+            const int c = 4 * lane, n = n0 + c;
+            if (n < g.N) {
+                uint32_t peer[8];
+#pragma unroll
+                for (int s = 0; s < 8; ++s) {
+                    peer[s] = 0;
+                    if (s < S) asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(peer[s]) : "r"(base + 4u * c), "r"(s));
+                }
+                float bias_n[4];
+#pragma unroll
+                for (int e = 0; e < 4; ++e) bias_n[e] = (g.bias && !g.bias_on_m && n + e < g.N) ? g.bias[n + e] : 0.f;
+#pragma unroll 1
+                for (int m = (int)rank + S * warp; m < g.M; m += 4 * S) {
+                    if (g.row_mask && g.row_mask[m] == 0) continue;
+                    float x[4][8];
+#pragma unroll
+                    for (int s = 0; s < 8; ++s) {
+                        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+                        if (s < S)
+                            asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];"
+                                         : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+                                         : "r"(peer[s] + (uint32_t)(m * PART_LD * 4)));
+                        x[0][s] = v.x; x[1][s] = v.y; x[2][s] = v.z; x[3][s] = v.w;
+                    }
+#pragma unroll
+                    for (int e = 0; e < 4; ++e)
+                        if (n + e < g.N) split_epilogue_one(g, m, n + e, x[e], bias_n[e]);
                 }
             }
         }
@@ -446,12 +605,18 @@ int gemm_tc_launch(const WtsGemm& g, cudaStream_t st)
     if (n_sm == 0) {
         WTS_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GT_SMEM));
         WTS_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_skinny_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GT_SMEM));
+        WTS_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_skinny64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SK_SMEM));
         int dev = 0;
         WTS_CUDA_CHECK(cudaGetDevice(&dev));
         WTS_CUDA_CHECK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
     }
+    const int tiles_n = (g.N + BN - 1) / BN, tiles_m = (g.M + BM - 1) / BM, nkb = (g.K + BK - 1) / BK;
+    const int batch = g.batch_outer * g.batch_inner;
+    const bool skinny = tiles_m == 1 && batch == 1 && g.head_dim == 0;
+    const bool skinny64 = skinny && g.M <= SK_BM;
     alignas(64) CUtensorMap tmA, tmB;
-    int rc = make_map(&tmA, g.a, g.K, g.M, g.lda, g.a_plane, g.batch_inner, g.a_bi, g.batch_outer, g.a_bo, BM, "A");
+    int rc = make_map(&tmA, g.a, g.K, g.M, g.lda, g.a_plane, g.batch_inner, g.a_bi, g.batch_outer, g.a_bo,
+                      skinny64 ? SK_BM : BM, "A");
     if (rc) return rc;
     rc = make_map(&tmB, g.b, g.K, g.N, g.ldb, g.b_plane, g.batch_inner, g.b_bi, g.batch_outer, g.b_bo, BN, "B");
     if (rc) return rc;
@@ -459,12 +624,9 @@ int gemm_tc_launch(const WtsGemm& g, cudaStream_t st)
     args.g = g;
     args.a_has_bo = g.a_bo != 0; args.a_has_bi = g.a_bi != 0;
     args.b_has_bo = g.b_bo != 0; args.b_has_bi = g.b_bi != 0;
-    const int tiles_n = (g.N + BN - 1) / BN, tiles_m = (g.M + BM - 1) / BM, nkb = (g.K + BK - 1) / BK;
-    const int batch = g.batch_outer * g.batch_inner;
     cudaLaunchConfig_t cfg = {};
     cfg.dynamicSmemBytes = GT_SMEM;
     cfg.stream = st;
-    const bool skinny = tiles_m == 1 && batch == 1 && g.head_dim == 0;
     if (!skinny) {
         const int64_t tiles = (int64_t)tiles_m * tiles_n * batch;
         if (tiles > INT32_MAX / 2) { set_error("wts_gemm(tc): %lld output tiles are too many", (long long)tiles); return -7; }
@@ -491,7 +653,8 @@ int gemm_tc_launch(const WtsGemm& g, cudaStream_t st)
     args.split_k = split;
     args.pair_stores = 0;
     cfg.gridDim = dim3(tiles_n, 1, split);
-    cfg.blockDim = dim3(GT_THREADS, 1, 1);
+    cfg.blockDim = dim3(skinny64 ? SK_THREADS : GT_THREADS, 1, 1);
+    if (skinny64) cfg.dynamicSmemBytes = SK_SMEM;
     cudaLaunchAttribute attr[2];
     int na = 0;
     if (split > 1) {
@@ -508,7 +671,8 @@ int gemm_tc_launch(const WtsGemm& g, cudaStream_t st)
     }
     cfg.attrs = attr;
     cfg.numAttrs = na;
-    WTS_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_tc_skinny_kernel, tmA, tmB, args));
+    if (skinny64) WTS_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_tc_skinny64_kernel, tmA, tmB, args));
+    else WTS_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_tc_skinny_kernel, tmA, tmB, args));
     return 0;
 }
 

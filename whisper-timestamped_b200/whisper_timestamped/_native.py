@@ -49,7 +49,7 @@ class Gemm(ctypes.Structure):
         ("out_sb16", ctypes.c_void_p), ("ldo", ctypes.c_int64), ("o_plane", ctypes.c_int64), ("o_bo", ctypes.c_int64), ("o_bi", ctypes.c_int64),
         ("head_dim", ctypes.c_int32), ("head_stride", ctypes.c_int64),
         ("backend", ctypes.c_int32), ("a_is_f32", ctypes.c_int32), ("b_is_f32", ctypes.c_int32),
-        ("row_mask", ctypes.c_void_p),
+        ("row_mask", ctypes.c_void_p), ("b_const", ctypes.c_int32),
     ]
 
 

@@ -124,8 +124,10 @@ class CudaEngine:
              batch=(1, 1), a_b=(0, 0), b_b=(0, 0), alpha=1.0, bias=None, bias_on_m=False, act=0,
              residual=None, ldr=0, r_b=(0, 0), out_f32=None, ldc=0, c_b=(0, 0), c_off=0,
              out_sb=None, ldo=0, o_plane=0, o_b=(0, 0), o_off=0, head_dim=0, head_stride=0,
-             a_f32=False, b_f32=False, backend=None, row_mask=None):
-        """a/b: SB16 objects (or float32 tensors with a_f32/b_f32).  Offsets/strides in elements."""
+             a_f32=False, b_f32=False, backend=None, row_mask=None, b_const=False):
+        """a/b: SB16 objects (or float32 tensors with a_f32/b_f32).  Offsets/strides in elements.  b_const: b is a model
+        weight that no kernel of the stream writes, so a decode-time GEMM may start loading it before the previous
+        kernel has completed."""
         g = nat.Gemm()
         if a_f32:
             g.a, g.lda, g.a_plane = a.data_ptr() + 4 * a_off, lda, 0
@@ -156,6 +158,7 @@ class CudaEngine:
         g.backend = self.backend if backend is None else backend
         g.a_is_f32, g.b_is_f32 = int(a_f32), int(b_f32)
         g.row_mask = row_mask.data_ptr() if row_mask is not None else None
+        g.b_const = int(b_const)
         if a_f32 or b_f32:
             g.backend = 1
         nat.check(nat.lib.wts_gemm(ctypes.byref(g), self._st()), "wts_gemm")
@@ -291,7 +294,7 @@ class CudaEngine:
             s0, n_l = self.layer_slots[li]
             kal = st8["ckal"][li]
             self.layernorm(x, a.ln_g, a.ln_b, R, D, out_sb=hs)
-            self.gemm(hs, a.qkv, R, 3 * D, D, bias=a.qkv_b, out_f32=qkv, ldc=3 * D, row_mask=active)
+            self.gemm(hs, a.qkv, R, 3 * D, D, bias=a.qkv_b, out_f32=qkv, ldc=3 * D, row_mask=active, b_const=True)
             fused_append = active is not None          # decode step: one row per sequence, the attention CTA appends K/V
             if not fused_append:
                 nat.check(nat.lib.wts_kv_append(qkv.data_ptr() + 4 * D, qkv.data_ptr() + 8 * D, 3 * D, row_seq.data_ptr(),
@@ -304,18 +307,21 @@ class CudaEngine:
                                                     att.plane, None, None, 0, 0, None,
                                                     active.data_ptr() if active is not None else None, st),
                       "wts_decoder_attention")
-            self.gemm(att, a.out, R, D, D, bias=a.out_b, residual=x, ldr=D, out_f32=x, ldc=D, row_mask=active)
+            self.gemm(att, a.out, R, D, D, bias=a.out_b, residual=x, ldr=D, out_f32=x, ldc=D, row_mask=active,
+                      b_const=True)
             self.layernorm(x, c.ln_g, c.ln_b, R, D, out_sb=hs)
-            self.gemm(hs, c.q, R, D, D, bias=c.q_b, out_f32=q, ldc=D, row_mask=active)
+            self.gemm(hs, c.q, R, D, D, bias=c.q_b, out_f32=q, ldc=D, row_mask=active, b_const=True)
             nat.check(nat.lib.wts_cross_attention_f16_layer(
                 q.data_ptr(), D, st8["ck"][li].data_ptr(), st8["cv"][li].data_ptr(), kal.data_ptr() if kal is not None else None,
                 self.head_slot[li].data_ptr(), n_slots, s0, n_l, N_CTX_AUDIO, row_seq.data_ptr(), R, H, att.ptr, att.ld,
                 att.plane, qk_buf.data_ptr(), qk_buf.shape[2], qk_row.data_ptr(),
                 active.data_ptr() if active is not None else None, st), "wts_cross_attention_f16_layer")
-            self.gemm(att, c.out, R, D, D, bias=c.out_b, residual=x, ldr=D, out_f32=x, ldc=D, row_mask=active)
+            self.gemm(att, c.out, R, D, D, bias=c.out_b, residual=x, ldr=D, out_f32=x, ldc=D, row_mask=active,
+                      b_const=True)
             self.layernorm(x, blk.mlp_ln_g, blk.mlp_ln_b, R, D, out_sb=hs)
-            self.gemm(hs, blk.fc1, R, 4 * D, D, bias=blk.fc1_b, act=1, out_sb=mid, row_mask=active)
-            self.gemm(mid, blk.fc2, R, D, 4 * D, bias=blk.fc2_b, residual=x, ldr=D, out_f32=x, ldc=D, row_mask=active)
+            self.gemm(hs, blk.fc1, R, 4 * D, D, bias=blk.fc1_b, act=1, out_sb=mid, row_mask=active, b_const=True)
+            self.gemm(mid, blk.fc2, R, D, 4 * D, bias=blk.fc2_b, residual=x, ldr=D, out_f32=x, ldc=D, row_mask=active,
+                      b_const=True)
             self.launches += 2
 
     def _alloc_decoder_state(self, B, R):
@@ -367,7 +373,7 @@ class CudaEngine:
         if hs is None:
             hs = SB16(n_rows, D, self.dev)
         self.layernorm(x_rows, w.ln_g, w.ln_b, n_rows, D, out_sb=hs)
-        self.gemm(hs, w.emb_sb, n_rows, V, D, out_f32=logits, ldc=V, row_mask=row_mask)
+        self.gemm(hs, w.emb_sb, n_rows, V, D, out_f32=logits, ldc=V, row_mask=row_mask, b_const=True)
 
     def decode_windows(self, jobs, setup):
         if getattr(setup, "beam_size", None) is not None or setup.temperature > 0:
