@@ -1,8 +1,8 @@
-"""The decode-time GEMM of a session of at most 64 windows (gemm_tc_skinny64_kernel: one 64-row A box, weights fetched
-before the dependency wait) against the 128-row kernel it replaces there, bit for bit, and against a float64 product.
+"""The decode-time GEMM of a session of at most 64 windows (gemm_tc_split_kernel<1>: one 64-row A box, weights fetched
+before the dependency wait) against the 128-row instance, bit for bit, and against a float64 product.
 
-The 128-row kernel (gemm_tc_skinny_kernel) still runs every one-tile GEMM of 65..128 rows, so the same rows padded to
-M = 65 with zero rows (masked) give the old arithmetic to compare with."""
+The 128-row instance (gemm_tc_split_kernel<2>) runs every one-tile GEMM of 65..128 rows, so the same rows padded to
+M = 65 with zero rows (masked) give its arithmetic to compare with."""
 import gc
 
 import numpy as np

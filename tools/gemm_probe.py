@@ -7,6 +7,9 @@ of dependent launches (what the decode step does), so host launch cost does not 
 `encoder`: every GEMM the large-v3 encoder and the cross-K/V projection issue for a batch of --windows 30-s windows
 (operand layouts and epilogues as engine.encode / engine._cross_kv issue them), the bench's roofline shape, and a bf16
 torch.matmul at the fc1 shape (the dense rate the card reaches; a third of it bounds the 3-term split-bf16 product).
+`skinny`: every GEMM of a large-v3 decode step (qkv, out-projection with in-place residual, fc1 with GELU and SB16
+output, fc2 with in-place residual, vocabulary projection with a row mask) at M = 1, 9, 64 (the 64-row instance of the
+split-K kernel) and 65, 128 (the 128-row one), timed as a graph chain over distinct weight sets.
 Each GEMM first runs once on seeded inputs and its output is digested on the device; --json writes the digests and
 times, --compare checks them bit for bit against another build's --json (e.g. the parent commit's tree via --pkg)."""
 import argparse
@@ -130,6 +133,64 @@ def encoder_shapes(eng, B, dev, results):
     results.append(dict(name="torch.matmul bf16 (fc1 shape)", M=M, N=N, K=K, ms=ms, tflops=tf))
 
 
+def decode_shapes(eng, dev, results):
+    from whisper_timestamped.model import SB16
+    D, V = 1280, 51866
+    n_w = 24                          # distinct weight sets so the chain streams weights from HBM like the decode step
+    gen = torch.Generator(device=dev)
+
+    def sb(rows, cols, seed, std=1.0):
+        s = SB16(rows, cols, dev)
+        gen.manual_seed(seed)
+        s.t.normal_(0.0, std, generator=gen)
+        return s
+
+    def randn(shape, seed):
+        gen.manual_seed(seed)
+        return torch.randn(shape, device=dev, generator=gen)
+
+    # (name, N, K, epilogue), with the weights marked b_const as the engine's decode step issues them
+    shapes = [("dec qkv", 3 * D, D, "bias"), ("dec out +=x", D, D, "residual"), ("dec fc1 gelu sb16", 4 * D, D, "gelu"),
+              ("dec fc2 +=x", D, 4 * D, "residual"), ("dec vocab mask", V, D, "mask")]
+    for (name, N, K, epi) in shapes:
+        ws = [sb(N, K, 100 + i, 0.02) for i in range(n_w)]
+        bias = randn(N, 1) if epi != "mask" else None
+        for M in (1, 9, 64, 65, 128):
+            a = sb(M, K, 2)
+            mask = (torch.arange(M, device=dev) % 3 != 1).to(torch.int32) if epi == "mask" else None
+            if epi == "gelu":
+                out = SB16(M, N, dev)
+                res, kw = out.t, dict(act=1, out_sb=out)
+            else:
+                res = randn((M, N), 3)
+                kw = dict(out_f32=res, ldc=N, row_mask=mask)
+                if epi == "residual":
+                    kw.update(residual=res, ldr=N)
+
+            def chain(weights=ws):
+                for w in weights:
+                    eng.gemm(a, w, M, N, K, bias=bias, b_const=True, **kw)
+            chain(ws[:1])
+            torch.cuda.synchronize()
+            dig = _digest(res)
+            chain()
+            torch.cuda.synchronize()
+            graph = torch.cuda.CUDAGraph()
+            s = torch.cuda.Stream(device=dev)
+            s.wait_stream(torch.cuda.current_stream(dev))
+            with torch.cuda.stream(s):
+                with torch.cuda.graph(graph, stream=s):
+                    chain()
+            torch.cuda.current_stream(dev).wait_stream(s)
+            ms = _time(graph.replay, 10) / n_w
+            print(f"{name:17s} M={M:3d} N={N:5d} K={K:4d}: {ms * 1e3:7.2f} us per GEMM in a graph chain "
+                  f"(weights {4.0 * N * K / 1e6:.1f} MB -> {4.0 * N * K / ms / 1e9:.2f} TB/s)", flush=True)
+            results.append(dict(name=f"{name} M={M}", M=M, N=N, K=K, ms=ms, digest=dig))
+            del graph
+        del ws
+        torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("which", nargs="?", default="all", choices=["all", "big", "skinny", "encoder"])
@@ -159,45 +220,8 @@ def main():
         print(f"encoder + cross-K/V GEMMs, large-v3, {args.windows} windows", flush=True)
         encoder_shapes(eng, args.windows, dev, results)
     if which in ("all", "skinny"):
-        n_w = 24                      # distinct weight sets so the chain streams weights from HBM like the decode step
-        for (M, N, K, name) in [(128, 1280, 1280, "dec out"), (128, 3840, 1280, "dec qkv"), (128, 5120, 1280, "dec fc1"),
-                                (128, 1280, 5120, "dec fc2"), (8, 1280, 1280, "dec out b8"), (8, 5120, 1280, "dec fc1 b8")]:
-            a = SB16(M, K, dev)
-            a.t.normal_()
-            ws = [SB16(N, K, dev) for _ in range(n_w)]
-            for w in ws:
-                w.t.normal_(0, 0.02)
-            bias = torch.zeros(N, device=dev)
-            x = torch.zeros(M, N, device=dev)
-            out = SB16(M, N, dev)
-
-            def chain():
-                for w in ws:
-                    if N == K:
-                        eng.gemm(a, w, M, N, K, bias=bias, residual=x, ldr=N, out_f32=x, ldc=N)
-                    else:
-                        eng.gemm(a, w, M, N, K, bias=bias, act=1, out_sb=out)
-            chain()
-            torch.cuda.synchronize()
-            graph = torch.cuda.CUDAGraph()
-            s = torch.cuda.Stream(device=dev)
-            s.wait_stream(torch.cuda.current_stream(dev))
-            with torch.cuda.stream(s):
-                with torch.cuda.graph(graph, stream=s):
-                    chain()
-            torch.cuda.current_stream(dev).wait_stream(s)
-            for _ in range(3):
-                graph.replay()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            torch.cuda.synchronize()
-            e0.record()
-            for _ in range(10):
-                graph.replay()
-            e1.record()
-            torch.cuda.synchronize()
-            us = e0.elapsed_time(e1) / 10 / n_w * 1e3
-            print(f"{name:11s} M={M} N={N} K={K}: {us:7.2f} us per GEMM in a graph chain "
-                  f"(weights {4.0 * N * K / 1e6:.1f} MB -> {4.0 * N * K / us / 1e6:.2f} TB/s)", flush=True)
+        print("decode-step GEMMs, large-v3", flush=True)
+        decode_shapes(eng, dev, results)
     if args.json:
         with open(args.json, "w") as f:
             json.dump(dict(device=torch.cuda.get_device_name(dev), windows=args.windows, results=results), f, indent=1)

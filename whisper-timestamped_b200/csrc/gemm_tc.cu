@@ -5,11 +5,11 @@
 // (the dropped lo*lo term is ~2^-16 relative).  That keeps logits and cross-attention scores within
 // the 1e-3 bar of the reference's float32 CPU path while running on the tensor cores.
 //
-// The first two kernels feed 128 x 128 output tiles from the same operand ring: per k-block the TMA producer lane loads 4 boxes
-// (A_hi, A_lo, B_hi, B_lo; 128 rows x 64 bf16, SWIZZLE_128B) into one of 3 stages; full[s] completes on the byte
-// count, empty[s] once the consumer warps have retired the k-block's wgmmas.  Batched problems (two batch levels) are
-// extra tensor-map dimensions; M/N/K tails rely on TMA zero fill.  Every output element sums the same k-blocks, k16
-// steps and terms (hi*hi, lo*hi, hi*lo) in the same order in every kernel here, so they give bit-identical results.
+// Both kernels feed 128-column output tiles from an operand ring: per k-block the TMA producer lane loads 4 boxes
+// (A_hi, A_lo, B_hi, B_lo; 64 bf16 wide, SWIZZLE_128B) into one ring stage; full[s] completes on the byte count,
+// empty[s] once the consumer warps have retired the k-block's wgmmas.  Batched problems (two batch levels) are extra
+// tensor-map dimensions; M/N/K tails rely on TMA zero fill.  Every output element sums the same k-blocks, k16 steps and
+// terms (hi*hi, lo*hi, hi*lo) in the same order in every kernel here, so they give bit-identical results.
 //
 // gemm_tc_kernel (encoder, cross-K/V, prefill: more than one M tile, batched, or head-major output): persistent,
 // warp-specialized, ping-pong.  grid = min(tiles, SMs), 384 threads:
@@ -20,24 +20,20 @@
 //                    ordered pair of named barriers makes the two main loops alternate, so one consumer's register-
 //                    direct epilogue runs while the other one's main loop holds the tensor cores.
 //
-// gemm_tc_skinny_kernel (decode time: one M tile, unbatched).  One CTA per 128-column tile, 288 threads: warpgroups 0, 1
-// consume rows 64*wg .. 64*wg+63 (one m64n128k16 x 3 terms per k16 step), warp 8 is the TMA lane.  These GEMMs are
-// weight-bandwidth bound, and with one CTA per 128-column tile too few SMs would stream the weights.  So K is split over
-// the CTAs of a thread-block CLUSTER (grid z = S, cluster = (1, 1, S), S <= 8): each CTA parks its float32 partial tile
-// in its own shared memory (the idle operand ring), the cluster synchronises, and CTA r reduces rows r, r + S, ... of
-// all S partials over distributed shared memory (ld.shared::cluster) and applies the epilogue to them: no atomics, no
-// global workspace, a fixed summation order (bit-reproducible), and the epilogue itself is spread over S SMs.
-//
-// gemm_tc_skinny64_kernel (the same with M <= 64: a decode step of a session of at most 64 windows).  One 64-row A box
-// (no wgmma on zero-filled rows), one consumer warpgroup plus the TMA warp (160 threads), a 4-stage ring of 48 KB stages.
-// A CTA streams only 2..10 k-blocks (20 for the vocabulary projection), so its time is round trips to HBM, not bytes.
-// With WtsGemm::b_const the producer issues the weight (B) boxes of all four ring stages before the dependency wait:
-// the whole share of a D x D GEMM's CTA and most of a QKV / FC1 CTA's are in flight while the previous kernel runs.
-// Split, k-block partition, wgmma sequence, partial-sum order and epilogue are those of gemm_tc_skinny_kernel: its rows
-// are bit-identical to the rows 0..63 of the 128-row kernel.
+// gemm_tc_split_kernel<WG> (decode time: one M tile, unbatched).  One CTA per 128-column tile: WG consumer warpgroups
+// read an A box of 64 * WG rows, warpgroup wg consumes rows 64*wg .. 64*wg+63 (one m64n128k16 x 3 terms per k16 step),
+// and warp 4 * WG is the TMA lane.  WG = 1 serves M <= 64 (a decode step of a session of at most 64 windows: no wgmma
+// on zero-filled rows) with a 4-stage ring of 48 KB stages, WG = 2 serves 65..128 rows with 3 stages of 64 KB.  These
+// GEMMs are weight-bandwidth bound, and with one CTA per 128-column tile too few SMs would stream the weights.  So K is
+// split over the CTAs of a thread-block CLUSTER (grid z = S, cluster = (1, 1, S), S <= 8): each CTA parks its float32
+// partial tile in its own shared memory (the idle operand ring), the cluster synchronises, and CTA r reduces rows
+// r, r + S, ... of all S partials over distributed shared memory (4 columns per 16-byte ld.shared::cluster) and applies
+// the epilogue to them: no atomics, no global workspace, a fixed summation order (bit-reproducible), and the epilogue
+// itself is spread over S SMs.  A CTA streams only 2..10 k-blocks (20 for the vocabulary projection), so its time is
+// round trips to HBM, not bytes: with WtsGemm::b_const the producer issues the weight (B) boxes of the first ring stages
+// before the dependency wait, so the whole share of a D x D GEMM's CTA and most of a QKV / FC1 CTA's are in flight while
+// the previous kernel runs.  Nothing of a row's arithmetic depends on WG: both instances give the same bits.
 #include <cuda_bf16.h>
-
-#include <stdlib.h>
 
 #include "sm90.cuh"
 
@@ -47,22 +43,23 @@ constexpr int BM = 128, BN = 128, BK = 64;
 constexpr int TILE_BYTES = BM * BK * 2;                 // 16 KB: one 128 x 64 bf16 box
 constexpr int STAGES = 3;
 constexpr int STAGE_BYTES = 4 * TILE_BYTES;
-constexpr int GT_THREADS = 288;                         // skinny kernel
 constexpr int PT_THREADS = 384;                         // persistent kernel: producer + 2 consumer warpgroups
 constexpr int PT_PRODUCER_REGS = 40, PT_CONSUMER_REGS = 232;
 static_assert(128 * PT_PRODUCER_REGS + 256 * PT_CONSUMER_REGS <= 65536, "setmaxnreg plan exceeds the register file");
 constexpr int GROUP_M = 8;                              // M tiles per raster group of the persistent scheduler
 constexpr int GT_SMEM = STAGES * STAGE_BYTES + 256 + 1024;
 constexpr int PART_LD = BN + 4;                         // float pitch of a parked partial tile
-static_assert(BM * PART_LD * 4 <= STAGES * STAGE_BYTES, "the partial tile lives in the operand ring");
-constexpr int SK_BM = 64;                               // one-tile variant: rows of its A box
-constexpr int SK_A_BYTES = SK_BM * BK * 2;              // 8 KB
-constexpr int SK_STAGES = 4;                            // measured: 2 and 3 stages are slower
-constexpr int SK_STAGE_BYTES = 2 * SK_A_BYTES + 2 * TILE_BYTES;   // A_hi, A_lo, B_hi, B_lo: 48 KB
-constexpr int SK_THREADS = 160;                         // one consumer warpgroup + the TMA warp
-constexpr int SK_SMEM = SK_STAGES * SK_STAGE_BYTES + 256 + 1024;
-static_assert(SK_BM * PART_LD * 4 <= SK_STAGES * SK_STAGE_BYTES, "the partial tile lives in the operand ring");
-static_assert(SK_SMEM <= 227 * 1024, "the 64-row kernel's ring fits in an SM's shared memory");
+
+// what differs between the two instances of gemm_tc_split_kernel
+template <int WG>
+struct SplitTraits {
+    static constexpr int A_BYTES = 64 * WG * BK * 2;
+    static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * TILE_BYTES;   // A_hi, A_lo, B_hi, B_lo
+    static constexpr int STAGES = WG == 1 ? 4 : 3;      // measured for WG = 1: 2 and 3 stages are slower
+    static constexpr int THREADS = 128 * WG + 32;       // the consumer warpgroups + the TMA warp
+    static_assert(STAGES * STAGE_BYTES + 256 + 1024 == GT_SMEM, "a 192 KB ring: the persistent kernel's shared memory");
+    static_assert(64 * WG * PART_LD * 4 <= STAGES * STAGE_BYTES, "the partial tile lives in the operand ring");
+};
 
 __device__ __forceinline__ float gelu_erf_tc(float v) { return 0.5f * v * (1.0f + erff(v * 0.70710678118654752440f)); }
 
@@ -312,132 +309,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     }
 }
 
-__global__ void __launch_bounds__(GT_THREADS, 1)
-gemm_tc_skinny_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcArgs args)
+template <int WG>
+__global__ void __launch_bounds__(SplitTraits<WG>::THREADS, 1)
+gemm_tc_split_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcArgs args)
 {
+    using T = SplitTraits<WG>;
     extern __shared__ unsigned char smem_raw[];
     const WtsGemm& g = args.g;
     const uint32_t base = (smem_addr(smem_raw) + 1023u) & ~1023u;
-    const uint32_t bar = base + STAGES * STAGE_BYTES;   // full[s] at +8s, empty[s] at +32+8s
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int n0 = blockIdx.x * BN, m0 = blockIdx.y * BM;
-    const int S = args.split_k;
-    const int z = S > 1 ? 0 : blockIdx.z, zo = z / g.batch_inner, zi = z - zo * g.batch_inner;
-    const int nkb_all = (g.K + BK - 1) / BK;
-    const int part_k = S > 1 ? blockIdx.z : 0;
-    const int kb0 = (int)((int64_t)part_k * nkb_all / S);
-    const int nkb = (int)((int64_t)(part_k + 1) * nkb_all / S) - kb0;
-    pdl_launch();
-
-    if (threadIdx.x == 256) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
-        for (int s = 0; s < STAGES; ++s) { mbar_init(bar + 8 * s, 1); mbar_init(bar + 32 + 8 * s, 8); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    pdl_wait();                                     // everything above overlapped the previous kernel's tail
-
-    float acc[64];
-    if (warp == 8) {
-        if (lane == 0) {
-            const int azo = args.a_has_bo ? zo : 0, azi = args.a_has_bi ? zi : 0;
-            const int bzo = args.b_has_bo ? zo : 0, bzi = args.b_has_bi ? zi : 0;
-            for (int kb = 0; kb < nkb; ++kb) {
-                const int s = kb % STAGES, u = kb / STAGES;
-                mbar_wait(bar + 32 + 8 * s, (u & 1) ^ 1);
-                const uint32_t full = bar + 8 * s;
-                mbar_expect_tx(full, STAGE_BYTES);
-                const uint32_t st = base + s * STAGE_BYTES;
-                const int kc = (kb0 + kb) * BK;
-                tma_load_5d(st, &tmA, full, kc, m0, azi, azo, 0);
-                tma_load_5d(st + TILE_BYTES, &tmA, full, kc, m0, azi, azo, 1);
-                tma_load_5d(st + 2 * TILE_BYTES, &tmB, full, kc, n0, bzi, bzo, 0);
-                tma_load_5d(st + 3 * TILE_BYTES, &tmB, full, kc, n0, bzi, bzo, 1);
-            }
-        }
-    } else {
-        const int wg = warp >> 2;
-#pragma unroll
-        for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-        for (int kb = 0; kb < nkb; ++kb) {
-            const int s = kb % STAGES, u = kb / STAGES;
-            mbar_wait(bar + 8 * s, u & 1);
-            const uint32_t st = base + s * STAGE_BYTES;
-            const uint64_t a_hi = wg_desc(st + wg * (TILE_BYTES / 2)), a_lo = wg_desc(st + TILE_BYTES + wg * (TILE_BYTES / 2));
-            const uint64_t b_hi = wg_desc(st + 2 * TILE_BYTES), b_lo = wg_desc(st + 3 * TILE_BYTES);
-            wg_fence();
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k) {
-                const uint64_t adv = (uint64_t)(k * 2);       // 32 bytes per K=16 step, in 16-byte units
-                wgmma_ss_n128(acc, a_hi + adv, b_hi + adv, 1);
-                wgmma_ss_n128(acc, a_lo + adv, b_hi + adv, 1);
-                wgmma_ss_n128(acc, a_hi + adv, b_lo + adv, 1);
-            }
-            wg_commit();
-            wg_wait<1>();                                     // the previous k-block's wgmmas have retired
-            if (kb > 0 && lane == 0) mbar_arrive(bar + 32 + 8 * ((kb - 1) % STAGES));
-        }
-        wg_wait<0>();
-
-        const int rl = 64 * wg + 16 * (warp & 3) + (lane >> 2);   // tile row of acc[4j + 0/1]; acc[4j + 2/3]: rl + 8
-        const int cl = 2 * (lane & 3);                            // tile column of acc[4j]: cl + 8j
-        if (S == 1) {
-            epilogue_frag64<false>(g, zo, zi, m0 + 64 * wg + 16 * (warp & 3), n0, acc);
-        } else {
-            // the ring is idle once BOTH warpgroups have retired their wgmmas (every TMA write has landed: all full
-            // barriers were waited)
-            asm volatile("bar.sync 1, 256;" ::: "memory");
-            float* part = reinterpret_cast<float*>(smem_raw + (base - smem_addr(smem_raw)));
-#pragma unroll
-            for (int i = 0; i < 2; ++i)
-#pragma unroll
-                for (int j = 0; j < 16; ++j)
-                    *reinterpret_cast<float2*>(part + (rl + 8 * i) * PART_LD + cl + 8 * j) =
-                        make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
-        }
-    }
-    if (S > 1) {
-        __syncwarp();
-        cluster_sync_all();                          // every partial tile is parked and visible cluster-wide
-        if (threadIdx.x < 256) {
-            uint32_t rank;
-            asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(rank));
-            const int c = threadIdx.x & 127, half = threadIdx.x >> 7;
-            const int n = n0 + c;
-            if (n < g.N) {
-                uint32_t peer[8];
-#pragma unroll
-                for (int s = 0; s < 8; ++s) {
-                    peer[s] = 0;
-                    if (s < S) asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(peer[s]) : "r"(base + 4u * c), "r"(s));
-                }
-                const float bias_n = (g.bias && !g.bias_on_m) ? g.bias[n] : 0.f;
-#pragma unroll 1
-                for (int m = (int)rank + S * half; m < g.M; m += 2 * S) {
-                    if (g.row_mask && g.row_mask[m] == 0) continue;
-                    float x[8];
-#pragma unroll
-                    for (int s = 0; s < 8; ++s) {
-                        x[s] = 0.f;
-                        if (s < S) asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(x[s]) : "r"(peer[s] + (uint32_t)(m * PART_LD * 4)));
-                    }
-                    split_epilogue_one(g, m, n, x, bias_n);
-                }
-            }
-        }
-        __syncwarp();
-        cluster_sync_all();                          // nobody leaves while a peer may still read its partial tile
-    }
-}
-
-__global__ void __launch_bounds__(SK_THREADS, 1)
-gemm_tc_skinny64_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcArgs args)
-{
-    extern __shared__ unsigned char smem_raw[];
-    const WtsGemm& g = args.g;
-    const uint32_t base = (smem_addr(smem_raw) + 1023u) & ~1023u;
-    const uint32_t bar = base + SK_STAGES * SK_STAGE_BYTES;   // full[s] at +8s, empty[s] at +32+8s
+    const uint32_t bar = base + T::STAGES * T::STAGE_BYTES;   // full[s] at +8s, empty[s] at +32+8s
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n0 = blockIdx.x * BN;
     const int S = args.split_k;
@@ -446,57 +326,59 @@ gemm_tc_skinny64_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
     const int nkb = (int)((int64_t)(blockIdx.z + 1) * nkb_all / S) - kb0;
     pdl_launch();
 
-    if (threadIdx.x == 128) {
+    if (threadIdx.x == 128 * WG) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
-        for (int s = 0; s < SK_STAGES; ++s) { mbar_init(bar + 8 * s, 1); mbar_init(bar + 32 + 8 * s, 4); }
+        for (int s = 0; s < T::STAGES; ++s) { mbar_init(bar + 8 * s, 1); mbar_init(bar + 32 + 8 * s, 4 * WG); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
 
     float acc[64];
-    if (warp == 4) {
+    if (warp == 4 * WG) {
         if (lane == 0) {
             // the weights are not written by any earlier kernel of the stream: the first stages' B boxes are issued
             // before the dependency wait, their A (activation) boxes after it, on the same full barriers
-            const int pre = g.b_const ? min(nkb, SK_STAGES) : 0;
+            const int pre = g.b_const ? min(nkb, T::STAGES) : 0;
             for (int kb = 0; kb < pre; ++kb) {
-                const uint32_t st = base + kb * SK_STAGE_BYTES, full = bar + 8 * kb;
-                mbar_expect_tx(full, SK_STAGE_BYTES);
-                tma_load_5d(st + 2 * SK_A_BYTES, &tmB, full, (kb0 + kb) * BK, n0, 0, 0, 0);
-                tma_load_5d(st + 2 * SK_A_BYTES + TILE_BYTES, &tmB, full, (kb0 + kb) * BK, n0, 0, 0, 1);
+                const uint32_t st = base + kb * T::STAGE_BYTES, full = bar + 8 * kb;
+                mbar_expect_tx(full, T::STAGE_BYTES);
+                tma_load_5d(st + 2 * T::A_BYTES, &tmB, full, (kb0 + kb) * BK, n0, 0, 0, 0);
+                tma_load_5d(st + 2 * T::A_BYTES + TILE_BYTES, &tmB, full, (kb0 + kb) * BK, n0, 0, 0, 1);
             }
             pdl_wait();
             for (int kb = 0; kb < pre; ++kb) {
-                const uint32_t st = base + kb * SK_STAGE_BYTES, full = bar + 8 * kb;
+                const uint32_t st = base + kb * T::STAGE_BYTES, full = bar + 8 * kb;
                 tma_load_5d(st, &tmA, full, (kb0 + kb) * BK, 0, 0, 0, 0);
-                tma_load_5d(st + SK_A_BYTES, &tmA, full, (kb0 + kb) * BK, 0, 0, 0, 1);
+                tma_load_5d(st + T::A_BYTES, &tmA, full, (kb0 + kb) * BK, 0, 0, 0, 1);
             }
             for (int kb = pre; kb < nkb; ++kb) {
-                const int s = kb % SK_STAGES, u = kb / SK_STAGES;
+                const int s = kb % T::STAGES, u = kb / T::STAGES;
                 mbar_wait(bar + 32 + 8 * s, (u & 1) ^ 1);
                 const uint32_t full = bar + 8 * s;
-                mbar_expect_tx(full, SK_STAGE_BYTES);
-                const uint32_t st = base + s * SK_STAGE_BYTES;
+                mbar_expect_tx(full, T::STAGE_BYTES);
+                const uint32_t st = base + s * T::STAGE_BYTES;
                 const int kc = (kb0 + kb) * BK;
                 tma_load_5d(st, &tmA, full, kc, 0, 0, 0, 0);
-                tma_load_5d(st + SK_A_BYTES, &tmA, full, kc, 0, 0, 0, 1);
-                tma_load_5d(st + 2 * SK_A_BYTES, &tmB, full, kc, n0, 0, 0, 0);
-                tma_load_5d(st + 2 * SK_A_BYTES + TILE_BYTES, &tmB, full, kc, n0, 0, 0, 1);
+                tma_load_5d(st + T::A_BYTES, &tmA, full, kc, 0, 0, 0, 1);
+                tma_load_5d(st + 2 * T::A_BYTES, &tmB, full, kc, n0, 0, 0, 0);
+                tma_load_5d(st + 2 * T::A_BYTES + TILE_BYTES, &tmB, full, kc, n0, 0, 0, 1);
             }
         } else {
             pdl_wait();
         }
     } else {
         pdl_wait();                                 // the epilogue reads bias / residual / row mask written upstream
+        // the warpgroup's 64 rows of an A box; a literal 0 for WG = 1, where the compiler cannot infer warp < 4
+        const uint32_t a_rows = (WG == 1 ? 0 : warp >> 2) * (T::A_BYTES / WG);
 #pragma unroll
         for (int i = 0; i < 64; ++i) acc[i] = 0.f;
         for (int kb = 0; kb < nkb; ++kb) {
-            const int s = kb % SK_STAGES, u = kb / SK_STAGES;
+            const int s = kb % T::STAGES, u = kb / T::STAGES;
             mbar_wait(bar + 8 * s, u & 1);
-            const uint32_t st = base + s * SK_STAGE_BYTES;
-            const uint64_t a_hi = wg_desc(st), a_lo = wg_desc(st + SK_A_BYTES);
-            const uint64_t b_hi = wg_desc(st + 2 * SK_A_BYTES), b_lo = wg_desc(st + 2 * SK_A_BYTES + TILE_BYTES);
+            const uint32_t st = base + s * T::STAGE_BYTES;
+            const uint64_t a_hi = wg_desc(st + a_rows), a_lo = wg_desc(st + T::A_BYTES + a_rows);
+            const uint64_t b_hi = wg_desc(st + 2 * T::A_BYTES), b_lo = wg_desc(st + 2 * T::A_BYTES + TILE_BYTES);
             wg_fence();
 #pragma unroll
             for (int k = 0; k < BK / 16; ++k) {
@@ -507,15 +389,16 @@ gemm_tc_skinny64_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
             }
             wg_commit();
             wg_wait<1>();                                     // the previous k-block's wgmmas have retired
-            if (kb > 0 && lane == 0) mbar_arrive(bar + 32 + 8 * ((kb - 1) % SK_STAGES));
+            if (kb > 0 && lane == 0) mbar_arrive(bar + 32 + 8 * ((kb - 1) % T::STAGES));
         }
         wg_wait<0>();
 
         if (S == 1) {
             epilogue_frag64<false>(g, 0, 0, 16 * warp, n0, acc);
         } else {
-            // every TMA write has landed (all full barriers were waited) and every wgmma has retired: the ring is idle
-            asm volatile("bar.sync 1, 128;" ::: "memory");
+            // the ring is idle once every consumer warpgroup has retired its wgmmas (every TMA write has landed: all
+            // full barriers were waited)
+            asm volatile("bar.sync 1, %0;" ::"n"(128 * WG) : "memory");
             float* part = reinterpret_cast<float*>(smem_raw + (base - smem_addr(smem_raw)));
             const int rl = 16 * warp + (lane >> 2), cl = 2 * (lane & 3);
 #pragma unroll
@@ -529,9 +412,9 @@ gemm_tc_skinny64_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
     if (S > 1) {
         __syncwarp();
         cluster_sync_all();                          // every partial tile is parked and visible cluster-wide
-        if (threadIdx.x < 128) {
-            // CTA r reduces rows r + S * (4i + warp); a lane owns 4 adjacent columns and reads them from each of
-            // the S partial tiles with one 16-byte distributed-shared-memory load
+        if (threadIdx.x < 128 * WG) {
+            // CTA r reduces rows r + S * (4 * WG * i + warp); a lane owns 4 adjacent columns and reads them from each
+            // of the S partial tiles with one 16-byte distributed-shared-memory load
             uint32_t rank;
             asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(rank));
             const int c = 4 * lane, n = n0 + c;
@@ -546,7 +429,7 @@ gemm_tc_skinny64_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
 #pragma unroll
                 for (int e = 0; e < 4; ++e) bias_n[e] = (g.bias && !g.bias_on_m && n + e < g.N) ? g.bias[n + e] : 0.f;
 #pragma unroll 1
-                for (int m = (int)rank + S * warp; m < g.M; m += 4 * S) {
+                for (int m = (int)rank + S * warp; m < g.M; m += 4 * WG * S) {
                     if (g.row_mask && g.row_mask[m] == 0) continue;
                     float x[4][8];
 #pragma unroll
@@ -603,9 +486,8 @@ int gemm_tc_launch(const WtsGemm& g, cudaStream_t st)
 {
     static int n_sm = 0;
     if (n_sm == 0) {
-        WTS_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GT_SMEM));
-        WTS_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_skinny_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GT_SMEM));
-        WTS_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_skinny64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SK_SMEM));
+        for (auto kernel : {gemm_tc_kernel, gemm_tc_split_kernel<1>, gemm_tc_split_kernel<2>})
+            WTS_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GT_SMEM));
         int dev = 0;
         WTS_CUDA_CHECK(cudaGetDevice(&dev));
         WTS_CUDA_CHECK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
@@ -613,10 +495,10 @@ int gemm_tc_launch(const WtsGemm& g, cudaStream_t st)
     const int tiles_n = (g.N + BN - 1) / BN, tiles_m = (g.M + BM - 1) / BM, nkb = (g.K + BK - 1) / BK;
     const int batch = g.batch_outer * g.batch_inner;
     const bool skinny = tiles_m == 1 && batch == 1 && g.head_dim == 0;
-    const bool skinny64 = skinny && g.M <= SK_BM;
+    const int wg = g.M <= 64 ? 1 : 2;                 // consumer warpgroups of the split kernel
     alignas(64) CUtensorMap tmA, tmB;
     int rc = make_map(&tmA, g.a, g.K, g.M, g.lda, g.a_plane, g.batch_inner, g.a_bi, g.batch_outer, g.a_bo,
-                      skinny64 ? SK_BM : BM, "A");
+                      skinny ? 64 * wg : BM, "A");
     if (rc) return rc;
     rc = make_map(&tmB, g.b, g.K, g.N, g.ldb, g.b_plane, g.batch_inner, g.b_bi, g.batch_outer, g.b_bo, BN, "B");
     if (rc) return rc;
@@ -642,10 +524,8 @@ int gemm_tc_launch(const WtsGemm& g, cudaStream_t st)
         WTS_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel, tmA, tmB, args));
         return 0;
     }
-    // WTS_SPLITK=0 disables the K split of decode-time GEMMs
-    static const int splitk = []{ const char* e = getenv("WTS_SPLITK"); return e ? atoi(e) : 1; }();
     int split = 1;
-    if (splitk && 2 * tiles_n <= n_sm) {
+    if (2 * tiles_n <= n_sm) {
         split = n_sm / tiles_n;
         if (split > 8) split = 8;                     // portable cluster size
         if (split > nkb) split = nkb;
@@ -653,8 +533,7 @@ int gemm_tc_launch(const WtsGemm& g, cudaStream_t st)
     args.split_k = split;
     args.pair_stores = 0;
     cfg.gridDim = dim3(tiles_n, 1, split);
-    cfg.blockDim = dim3(skinny64 ? SK_THREADS : GT_THREADS, 1, 1);
-    if (skinny64) cfg.dynamicSmemBytes = SK_SMEM;
+    cfg.blockDim = dim3(wg == 1 ? SplitTraits<1>::THREADS : SplitTraits<2>::THREADS, 1, 1);
     cudaLaunchAttribute attr[2];
     int na = 0;
     if (split > 1) {
@@ -671,8 +550,7 @@ int gemm_tc_launch(const WtsGemm& g, cudaStream_t st)
     }
     cfg.attrs = attr;
     cfg.numAttrs = na;
-    if (skinny64) WTS_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_tc_skinny64_kernel, tmA, tmB, args));
-    else WTS_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_tc_skinny_kernel, tmA, tmB, args));
+    WTS_CUDA_CHECK(cudaLaunchKernelEx(&cfg, wg == 1 ? gemm_tc_split_kernel<1> : gemm_tc_split_kernel<2>, tmA, tmB, args));
     return 0;
 }
 
